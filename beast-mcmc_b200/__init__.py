@@ -1,4 +1,4 @@
-"""beast-mcmc_b200: a Blackwell-native (sm_100a) tree-likelihood engine that sits behind BEAST's
+"""beast-mcmc_b200: an H100-native (sm_90a) tree-likelihood engine that sits behind BEAST's
 BEAGLE boundary (libhmsbeagle C ABI + libhmsbeagle-jni JNI shim).
 
 The directory name carries a hyphen (as the project is named); import it as

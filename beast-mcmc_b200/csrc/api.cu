@@ -192,7 +192,7 @@ void buildResources() {
         snprintf(buf, sizeof buf, "%s", prop.name);
         gResourceStrings.push_back(buf);
         snprintf(buf, sizeof buf, "Global memory (MB): %zu | SMs: %d | compute capability: %d.%d | "
-                 "B200-native walk kernels (sm_100a), double precision",
+                 "native walk kernels (sm_90a), double precision",
                  (size_t)(prop.totalGlobalMem >> 20), prop.multiProcessorCount, prop.major, prop.minor);
         gResourceStrings.push_back(buf);
     }
@@ -213,7 +213,7 @@ void buildResources() {
     if (gShardDevices.size() > (size_t)kMaxGroup) gShardDevices.resize(kMaxGroup);
     if (!gShardDevices.empty()) {
         char buf[512];
-        snprintf(buf, sizeof buf, "B200 x %zu (pattern-sharded)", gShardDevices.size());
+        snprintf(buf, sizeof buf, "GPU x %zu (pattern-sharded)", gShardDevices.size());
         gResourceStrings.push_back(buf);
         snprintf(buf, sizeof buf, "one instance over %zu GPUs | contiguous pattern blocks (Patterns.java:142-169 rule) | "
                  "per-shard sums added over NVLink inside the root kernel", gShardDevices.size());
@@ -233,7 +233,7 @@ void buildResources() {
 }
 
 char gImplName[] = "B200-CUDA-Double";
-char gImplDesc[] = "sm_100a walk kernels: one launch per operation list, shared-memory operand stack";
+char gImplDesc[] = "sm_90a walk kernels: one launch per operation list, shared-memory operand stack";
 
 // ---- op planning ------------------------------------------------------------------------------
 
@@ -918,7 +918,7 @@ const char* beagleGetVersion(void) { return "4.0.1-b200+" B200_SOURCE_HASH; }
 const char* b200GetSourceHash(void) { return B200_SOURCE_HASH; }
 
 const char* beagleGetCitation(void) {
-    return "B200-native tree-likelihood engine exposing the BEAGLE API.\n"
+    return "H100-native tree-likelihood engine exposing the BEAGLE API.\n"
            "API after: Ayres et al. (2019) BEAGLE 3. Syst Biol 68:1052-1061.";
 }
 
@@ -1046,6 +1046,10 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->tensorR = envInt("B200_TENSOR_R", 2) >= 4 ? 4 : 2;
     in->genericMma = envInt("B200_GENERIC_MMA", 1);
     in->mmaWarps = envInt("B200_MMA_WARPS", 4) == 8 ? 8 : 4;     // 8 = 256-thread blocks with cp.async double buffering
+    // the SM count sizes the walk below: query the device first
+    cudaDeviceProp prop;
+    bool ok = cudaGetDeviceProperties(&prop, in->device) == cudaSuccess;
+    if (ok) { in->smCount = prop.multiProcessorCount; in->maxSmemOptin = prop.sharedMemPerBlockOptin; }
     in->walkR = envInt("B200_WALK_R", 4);
     if (in->walkR != 1 && in->walkR != 2 && in->walkR != 4 && in->walkR != 8) in->walkR = 4;
     if (getenv("B200_WALK_R") == nullptr && in->matCP > 0) {
@@ -1056,9 +1060,6 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     }
     in->stackDepthMax = std::min(64, std::max(0, envInt("B200_STACK_DEPTH", 12)));
 
-    cudaDeviceProp prop;
-    bool ok = cudaGetDeviceProperties(&prop, in->device) == cudaSuccess;
-    if (ok) { in->smCount = prop.multiProcessorCount; in->maxSmemOptin = prop.sharedMemPerBlockOptin; }
     ok = ok && cudaStreamCreateWithFlags(&in->stream, cudaStreamNonBlocking) == cudaSuccess;
     const size_t eigenStride = 2 * (size_t)in->S * in->S + 2 * in->S;
     const size_t matElems = (size_t)in->nMatrices * in->matStride;

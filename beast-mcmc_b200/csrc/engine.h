@@ -1,4 +1,4 @@
-// engine.h -- internal types of the B200 tree-likelihood engine (not part of the ABI).
+// engine.h -- internal types of the tree-likelihood engine (not part of the ABI).
 //
 // One Instance owns every device allocation between beagleCreateInstance and
 // beagleFinalizeInstance.  Device layout (DESIGN.md "Data layout in HBM"):
@@ -129,7 +129,7 @@ struct Instance {
     long flags = 0;
     bool logScalers = false, complexEigen = false;
     cudaStream_t stream = nullptr;
-    int smCount = 148;
+    int smCount = 132;                        // H100 SXM; replaced by the device's count at instance creation
     size_t maxSmemOptin = 0;
 
     size_t partialsElems = 0;                 // C*Ppad*Sp = stride of one partials slot

@@ -1,4 +1,4 @@
-// kernels.cu -- hand-written sm_100a kernels of the tree-likelihood hot path.
+// kernels.cu -- hand-written sm_90a kernels of the tree-likelihood hot path.
 //
 //   k_transition   : P_c(t) = Evec diag(exp(Eval r_c t)) Ievc           (updateTransitionMatrices)
 //   k_walk4        : 4-state (nucleotide) partials, WARP-OWNED PATTERN COLUMNS walking the whole
@@ -496,7 +496,7 @@ static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs
 //   A fragment = child partials  [8 patterns][4 states]   lane (g,t) <- X[p0+g][t]     (256 contiguous bytes / warp)
 //   B fragment = transition rows [4 (j)][8 (i)]            lane (g,t) <- Mpad[g][t]     (256 contiguous bytes, rows >= 4 zero)
 //   D fragment                    [8 patterns][8 (i)]      lane (g,t) -> i = 2t,2t+1 of pattern g (meaningful for t < 2)
-// tcgen05 has no fp64 kind, so the fp64 tensor path on sm_100a is mma.sync (SASS DMMA.8x8x4).
+// wgmma has no fp64 kind, so the fp64 tensor path on sm_90a is mma.sync (SASS DMMA.8x8x4).
 // The matrix reaches the register file ONCE per warp (8 B/lane) instead of once per thread (128 B/lane),
 // which is what saturates the LSU->RF path of the FMA kernel.  Everything is arranged so that loads need
 // no predicates: pattern rows are padded to 32, gap tips read a ones-column, B rows 4..7 are stored zeros;
@@ -811,6 +811,15 @@ __device__ __forceinline__ void cpAsync16(void* smemDst, const void* gmemSrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(s), "l"(gmemSrc) : "memory");
 }
 
+// x where `on`, else 0, as one selp the compiler cannot see through: a plain `on ? x : 0.0` ahead of an mma.sync lets it
+// specialise the mma per lane (zero operands folded, predicated copies), and mma.sync.aligned on diverged lanes deadlocks
+__device__ __forceinline__ double selOn(double x, bool on) {
+    double r;
+    asm volatile("{\n.reg .pred p;\nsetp.ne.u32 p, %2, 0;\nselp.f64 %0, %1, 0d0000000000000000, p;\n}\n"
+                 : "=d"(r) : "d"(x), "r"((unsigned)on));
+    return r;
+}
+
 // ---- TMA (1-D bulk copy) staging: one elected thread moves a whole padded matrix, completion on an mbarrier ----
 __device__ __forceinline__ void mbarInit(uint64_t* bar, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
@@ -921,14 +930,16 @@ k_walk_mma(const DevOp* __restrict__ ops, const int4* __restrict__ subs, int S, 
                 for (int m = 0; m < 2; ++m)
 #pragma unroll
                     for (int n = 0; n < NT; ++n) { u[m][n][0] = 0.0; u[m][n][1] = 0.0; }
-                const double* xrow0 = op.c2 + ((size_t)c * Ppad + (pw + g)) * Sp + t;
-                const double* xrow1 = xrow0 + (size_t)8 * Sp;
+                // mma.sync is .aligned: every lane must reach it on the same path.  Guarded loads let the compiler branch
+                // per lane (and deadlock a warp whose patterns straddle the end of the window), so every lane loads from
+                // a row clamped into the padded buffer and inactive lanes select zero (selOn).
+                const double* xrow0 = op.c2 + ((size_t)c * Ppad + min(pw + g, Ppad - 1)) * Sp + t;
+                const double* xrow1 = op.c2 + ((size_t)c * Ppad + min(pw + 8 + g, Ppad - 1)) * Sp + t;
                 const double* brow = P2 + g * LD + t;
 #pragma unroll 4
                 for (int kc = 0; kc < Sp / 4; ++kc) {
-                    double a0 = 0.0, a1 = 0.0;
-                    if (act[0]) a0 = xrow0[4 * kc];
-                    if (act[1]) a1 = xrow1[4 * kc];
+                    const double x0 = xrow0[4 * kc], x1 = xrow1[4 * kc];
+                    const double a0 = selOn(x0, act[0]), a1 = selOn(x1, act[1]);
 #pragma unroll
                     for (int n = 0; n < NT; ++n) {
                         const double b = brow[n * 8 * LD + 4 * kc];
@@ -1382,14 +1393,14 @@ k_edge_derivatives_mma(const EdgeRef* __restrict__ edges, const double* __restri
             for (int m = 0; m < 2; ++m)
 #pragma unroll
                 for (int n = 0; n < NT; ++n) { v[m][n][0] = 0.0; v[m][n][1] = 0.0; }
-            const double* xrow0 = e.post + ((size_t)c * Ppad + (pw + g)) * Sp + t;
-            const double* xrow1 = xrow0 + (size_t)8 * Sp;
+            // branch-free A operands ahead of the .aligned mma.sync: see the pre-order form of k_walk_mma
+            const double* xrow0 = e.post + ((size_t)c * Ppad + min(pw + g, Ppad - 1)) * Sp + t;
+            const double* xrow1 = e.post + ((size_t)c * Ppad + min(pw + 8 + g, Ppad - 1)) * Sp + t;
             const double* brow = smm + g * LD + t;
 #pragma unroll 4
             for (int kc = 0; kc < Sp / 4; ++kc) {
-                double a0 = 0.0, a1 = 0.0;
-                if (act[0]) a0 = xrow0[4 * kc];
-                if (act[1]) a1 = xrow1[4 * kc];
+                const double x0 = xrow0[4 * kc], x1 = xrow1[4 * kc];
+                const double a0 = selOn(x0, act[0]), a1 = selOn(x1, act[1]);
 #pragma unroll
                 for (int n = 0; n < NT; ++n) {
                     const double b = brow[n * 8 * LD + 4 * kc];

@@ -1,5 +1,5 @@
 // multi.cu -- the engine's own multi-GPU layer (SURVEY.md 8e, mode B): ONE BEAGLE instance whose site patterns are
-// sharded over several B200s of the node, so that an unmodified BEAST run (one likelihood, no -beagle_instances) uses
+// sharded over several GPUs of the node, so that an unmodified BEAST run (one likelihood, no -beagle_instances) uses
 // all of them by naming one resource ("-beagle_order <n+1>" on an n-GPU box, see buildResources in api.cu).
 //
 //   * sharding rule = the reference's own (-beagle_instances): contiguous blocks, floor(P/g) patterns each, the first

@@ -7,17 +7,18 @@ namespace b200 {
 // ---------------------------------------------------------------------------------------------
 // small device helpers
 // ---------------------------------------------------------------------------------------------
+// 32 contiguous bytes (one pattern's 4 states) as two 128-bit accesses: sm_90 has no 256-bit global load/store
 __device__ __forceinline__ void ldg256(const double* p, double (&v)[4]) {
-    asm volatile("ld.global.v4.f64 {%0,%1,%2,%3}, [%4];"
+    asm volatile("ld.global.v2.f64 {%0,%1}, [%4];\n\tld.global.v2.f64 {%2,%3}, [%4+16];"
                  : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "l"(p) : "memory");
 }
 // read-only path for data produced by an EARLIER launch (matrices)
 __device__ __forceinline__ void ldg256_nc(const double* p, double (&v)[4]) {
-    asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];"
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%4];\n\tld.global.nc.v2.f64 {%2,%3}, [%4+16];"
                  : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "l"(p));
 }
 __device__ __forceinline__ void stg256(double* p, const double (&v)[4]) {
-    asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};"
+    asm volatile("st.global.v2.f64 [%0], {%1,%2};\n\tst.global.v2.f64 [%0+16], {%3,%4};"
                  :: "l"(p), "d"(v[0]), "d"(v[1]), "d"(v[2]), "d"(v[3]) : "memory");
 }
 
@@ -57,7 +58,7 @@ __device__ __forceinline__ void prefetchL1(const void* p) {
 
 // non-volatile: a read-only load the scheduler may hoist freely
 __device__ __forceinline__ void ldg256_ro(const double* p, double (&v)[4]) {
-    asm("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];"
+    asm("ld.global.nc.v2.f64 {%0,%1}, [%4];\n\tld.global.nc.v2.f64 {%2,%3}, [%4+16];"
         : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "l"(p));
 }
 

@@ -1,7 +1,7 @@
 // walk4e.cu -- the 4-state (nucleotide) walk in EIGEN FORM: the default updatePartials kernel of S <= 4 instances.
 //
-// What bounded k_walk4 (profiles/r01_ncu_raw.txt, source page of the same capture): the L1/LSU data pipe at 70 % of peak
-// wavefronts, 60 % of them matrix traffic -- every thread needs its category's 4x4 matrix in registers (128 B per child)
+// What bounds k_walk4: the L1/LSU data pipe, most of it matrix traffic -- every thread needs its category's 4x4 matrix in
+// registers (128 B per child)
 // and a compact-tip child costs one 32-B matrix column per PATTERN -- while HBM only saw the mandatory destination writes.
 //
 // Here no transition matrix is read at all.  With one real eigen system per list (what HomogenousSubstitutionModelDelegate
@@ -223,8 +223,8 @@ k_walk4e(const WalkArgs A) {
 // ---------------------------------------------------------------------------------------------------------------------
 // k_walk4p -- the same arithmetic with PER-WARP ASYNCHRONOUS OPERAND STAGING (the default for aligned lists, CP <= 8).
 //
-// What bounded k_walk4e after the matrices were gone (profiles/r02_walk4e_summary.md): every pipe below 50 %, but 38 % of the
-// stall samples "long scoreboard" on first uses of small per-op operands -- the op record, the tips' state bytes, the
+// What bounds k_walk4e with the matrices gone: no pipe near its peak, but "long scoreboard" stalls on first uses of
+// small per-op operands -- the op record, the tips' state bytes, the
 // spectra, the P columns of tip children -- i.e. a chain of dependent L1/L2 latencies per op with 16 warps per SM to hide it.
 // Those operands are tiny, warp-uniform and known one op ahead, so each warp runs a two-deep cp.async (LDGSTS) pipeline into
 // its own slice of shared memory: while op k computes, record k+2 and ALL small operands of op k+1 travel global -> shared
@@ -235,8 +235,8 @@ k_walk4e(const WalkArgs A) {
 //                                            two half tables (states 0-1 / 2-3) of 16-byte entries indexed c*4 + j, so that
 //                                            the 8 lanes of a quarter warp (same category, 8 patterns) hit 4 distinct
 //                                            bank groups whatever their states -- with the HBM order kept ([j][c]: 128 B
-//                                            between states) they collided up to 4-way and 63 % of the kernel's shared-memory
-//                                            wavefronts were bank conflicts (profiles/r02_walk4e_summary.md).  Entries
+//                                            between states) they collided up to 4-way and most of the kernel's shared-memory
+//                                            wavefronts were bank conflicts.  Entries
 //                                            4*CP + c = the gap column (written once).  A pattern picks its column with two LDS.128
 //                      ev[child][CP][4]      spectrum of an internal child
 //                      st[child][G*R]        state bytes of a tip child for this warp's patterns
@@ -447,8 +447,8 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
     if constexpr (CP <= 8 && G * R >= 4) {
         if ((R == 1 ? in->thinTipMode : in->tipMode) == 3) {     // per-warp asynchronous operand staging (k_walk4p)
             if constexpr (CP == 4) {
-                // measured (profiles/r02_sweep_cfg2.txt): a launch bound of 3 blocks lets ptxas keep 120 registers without a
-                // spill and 4 blocks still fit -- the fastest setting unless B200_WALK_MINB says otherwise
+                // a launch bound of 3 blocks lets ptxas keep its registers without a spill and 4 blocks still fit -- the
+                // fastest setting where it was swept, unless B200_WALK_MINB says otherwise
                 const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;
                 if (minb >= 6) return launchP<CP, R, 6>(in, A, grid);
                 if (minb == 5) return launchP<CP, R, 5>(in, A, grid);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- tree log-likelihood evaluations/sec on B200 (BASELINE.json metric).
+"""bench.py -- tree log-likelihood evaluations/sec on H100 (BASELINE.json metric).
 
 A "step" is one full tree log-likelihood evaluation (all nodes dirty): the BEAGLE call sequence
 BeagleDataLikelihoodDelegate.calculateLikelihood issues (BDLD:812-937) --
@@ -7,10 +7,12 @@ setEigenDecomposition, setCategoryRates/Weights, setStateFrequencies, updateTran
 (2N-2 branches), updatePartials (N-1 operations), calculateRootLogLikelihoods -- through the C ABI
 of libhmsbeagle.so, with BEAST's double-buffer index flipping between steps.
 
-  value : K steps enqueued back to back on the instance stream (tip data / partials resident in HBM, result left on
-          the device), bracketed by barrier + synchronize, CUDA-event timed on the engine's stream, max over ranks.
-          The K-step block is repeated (>= 25 times, >= ~1 s in total) and the MEDIAN block is reported
-          (`repeats`, `block_ms_p10/p50/p90`): a 20-step block lasts 8 ms and one host hiccup would otherwise be the result.
+  value : after --warmup untimed steps, exactly --steps steps enqueued back to back on the instance stream (tip data /
+          partials resident in HBM, result left on the device), bracketed by barrier + synchronize, with a CUDA event
+          between consecutive steps; per-step times are the max over ranks, and the MEDIAN step is reported
+          (`repeats` = steps, `block_ms_p10/p50/p90` = per-step quantiles): one host hiccup cannot become the result.
+  --dump-outputs DIR : after the timed steps, what the last one computed (joint log-likelihood, per-pattern log-likelihoods,
+          root partials) as float64 .npy files, so that two builds can be compared output for output.
   e2e   : the same sequence through the synchronous reference-facing calls with HOST buffers:
           every step uploads the eigen system, rates, frequencies, branch lengths and op list and
           lands the 8-byte (joint) log-likelihood on the host; median per step, max over ranks.
@@ -31,11 +33,11 @@ from __future__ import annotations
 import argparse
 import ctypes as Cc
 import json
-import math
 import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -69,6 +71,11 @@ WORKLOADS = {
     "makona_like_1610x6k": dict(taxa=1610, patterns=6000, states=4, categories=4, rootHeight=0.0025, treeSeed=3),
 }
 FLU8_SITES = [2341, 2341, 2233, 1778, 1565, 1413, 1027, 890]      # SURVEY.md 8d cfg 5: segment-length-like site counts
+# roofline denominators: NVIDIA's H100 SXM data sheet (700 W card); a card set to a lower power limit reaches less
+H100_HBM_GBS = 3350.0                 # HBM3
+H100_FP64_TENSOR_TFLOPS = 67.0        # FP64 tensor core, dense (the DMMA pipe mma.sync m8n8k4 runs on)
+BENCH_CACHE = os.environ.get("B200_BENCH_CACHE", os.path.join(tempfile.gettempdir(), "b200_bench_cache"))
+DUMP_BYTES = 64 << 20                 # --dump-outputs: at most this much in all
 
 ZERO = np.zeros(1, dtype=np.int32)
 MINUS1 = np.full(1, -1, dtype=np.int32)
@@ -100,7 +107,7 @@ def build_workload(name, shard_index, overrides):
     site = em.GammaSiteRateModel(shape=0.5, gammaCategoryCount=w["categories"]) if w["categories"] > 1 \
         else em.GammaSiteRateModel()
     # the simulated alignment is cached per box (sweeps re-use it); it is regenerated when absent
-    cache = os.path.join(os.environ.get("B200_BENCH_CACHE", "/tmp/b200_bench_cache"),
+    cache = os.path.join(BENCH_CACHE,
                          f"{w.get('data', name)}_{w['taxa']}_{w['patterns']}_{w['states']}_{w['categories']}_{shard_index}.npz")
     if w.get("fixture"):
         z = np.load(os.path.join(ROOT, "tests", "golden", w["fixture"] + "_patterns.npz"))
@@ -203,15 +210,24 @@ def issue_sync(inst, ev, parity, out):
 # clocks
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi in loop mode (-lms) for the duration of the timed regions (B200_PROFILING.md clocks line)."""
+    """nvidia-smi in loop mode (-lms) for the duration of the timed regions, plus the card's name and power limit: an
+    absolute number is only meaningful next to what it was measured on."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown," \
         "clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index):
-        self.gpu_index, self.proc = gpu_index, None
+        self.gpu_index, self.proc, self.card = gpu_index, None, {"gpu": None, "power_limit_w": None}
 
     def start(self):
+        try:
+            row = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
+                                  "-i", str(self.gpu_index)], capture_output=True, text=True, timeout=30).stdout.strip()
+            if row.count(",") == 1:
+                name, limit = (c.strip() for c in row.split(","))
+                self.card = {"gpu": name, "power_limit_w": float(limit) if limit.replace(".", "").isdigit() else None}
+        except (OSError, subprocess.TimeoutExpired):
+            pass
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
                                           "-i", str(self.gpu_index), "-lms", "50"],
@@ -238,13 +254,18 @@ class ClockSampler:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
+        return {**self.card, "sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "power_w_max": max(pw) if pw else None, "reasons": sorted(reasons), "samples": len(rows)}
 
 
 # ------------------------------------------------------------------------------------------------
 # CPU arm (oracle port): cpu_baseline and --impl reference
 # ------------------------------------------------------------------------------------------------
+def usable_cores():
+    """CPUs this process may run on (a container or batch slot may allow fewer than the host has)."""
+    return len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
+
+
 def cpu_pick_threads(ev, S, C, P, cores):
     """The port's thread pool does not scale to every host (shared boxes, NUMA): try a few thread counts, five
     evaluations each, and keep the one with the best MEDIAN -- the baseline gets its best configuration."""
@@ -294,7 +315,7 @@ def run_reference_arm(args, meta_base):
     w, tree, pats, model, site = build_workload(args.workload, 0, vars(args))
     S, C, P = w["states"], site.getCategoryCount(), pats.patternCount
     ev = Evaluation(tree, pats, model, site, "POST_ORDER", scaling=bool(w.get("scaling")))
-    cores = os.cpu_count() or 1
+    cores = usable_cores()
     from oracle import cpu
     threads, tried = cpu_pick_threads(ev, S, C, P, cores)
     inst = create_instance(cpu.factory(threads=threads), ev, S, C, P, None)
@@ -384,38 +405,26 @@ def _quantiles(xs):
     return pick(0.10), pick(0.50), pick(0.90)
 
 
-def timed_blocks(D, stream, step_async, steps, warmup, min_repeats=25, min_total_s=1.0, max_repeats=400):
-    """K-step blocks, each bracketed by barrier + synchronize and timed with CUDA events on the engine's stream;
-    per-block max over ranks, then the quantiles over the blocks."""
+def timed_blocks(D, stream, step_async, steps, warmup):
+    """`warmup` untimed steps, then exactly `steps` steps back to back on the engine's stream, bracketed by barrier +
+    synchronize, with a CUDA event between consecutive steps; per-step max over ranks, then the quantiles over the steps
+    (every step is a block of one)."""
     torch = D.torch
     for k in range(max(3, warmup)):
         step_async(k)
     D.bracket()
-    # one pilot block decides how many repeats fill ~min_total_s
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(stream)
+    events = [torch.cuda.Event(enable_timing=True) for _ in range(steps + 1)]
+    t0 = time.perf_counter()
+    events[0].record(stream)
     for k in range(steps):
         step_async(k)
-    e1.record(stream)
+        events[k + 1].record(stream)
     D.bracket()
-    pilot = D.max_over_ranks([e0.elapsed_time(e1)])[0]
-    repeats = int(min(max_repeats, max(min_repeats, math.ceil(min_total_s * 1e3 / max(pilot, 1e-3)))))
-    blocks, walls = [], []
-    for _ in range(repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        D.bracket()
-        t0 = time.perf_counter()
-        a.record(stream)
-        for k in range(steps):
-            step_async(k)
-        b.record(stream)
-        D.bracket()
-        walls.append(time.perf_counter() - t0)
-        blocks.append(a.elapsed_time(b))
-    blocks = D.max_over_ranks(blocks)
-    p10, p50, p90 = _quantiles(blocks)
-    return {"repeats": repeats, "block_ms_p10": p10, "block_ms_p50": p50, "block_ms_p90": p90,
-            "wall_ms_per_step": 1e3 * statistics.median(walls) / steps}
+    wall = time.perf_counter() - t0
+    per = D.max_over_ranks([events[k].elapsed_time(events[k + 1]) for k in range(steps)])
+    p10, p50, p90 = _quantiles(per)
+    return {"repeats": steps, "block_ms_p10": p10, "block_ms_p50": p50, "block_ms_p90": p90,
+            "total_ms": events[0].elapsed_time(events[steps]), "wall_ms_per_step": 1e3 * wall / steps}
 
 
 def timed_e2e(D, step_e2e, steps):
@@ -443,7 +452,26 @@ def device_double(D, ptr, index=0):
     return D.torch.as_tensor(_Dev(), device=D.device)
 
 
-def measure_single_partition(D, lib, beagle, w, tree, pats, model, site, steps, warmup, kernel_timing=True, e2e_steps=None):
+def dump_outputs(directory, inst, ev, S, C, P, parity, joint):
+    """What the timed path's last step computed, as a caller of it would receive it: the joint log-likelihood, the
+    per-pattern log-likelihoods and the root partials (a fixed, seeded sample of patterns when they exceed the budget)."""
+    os.makedirs(directory, exist_ok=True)
+    site = np.zeros(P)
+    inst.getSiteLogLikelihoods(site)
+    root = np.zeros(C * P * S)
+    inst.getPartials(ev.rootIdx[parity], -1, root)
+    root = root.reshape(C, P, S)
+    keep = max(1, (DUMP_BYTES - 8 * P - 4096) // (8 * (C * S + 1)))
+    if keep < P:
+        pick = np.sort(np.random.default_rng(0).choice(P, keep, replace=False))
+        root = root[:, pick, :]
+        np.save(os.path.join(directory, "root_partials_patterns.npy"), pick.astype(np.float64))
+    np.save(os.path.join(directory, "log_likelihood.npy"), np.array([joint], dtype=np.float64))
+    np.save(os.path.join(directory, "site_log_likelihoods.npy"), site)
+    np.save(os.path.join(directory, "root_partials.npy"), np.ascontiguousarray(root))
+
+
+def measure_single_partition(D, lib, beagle, w, tree, pats, model, site, steps, warmup, kernel_timing=True, dump_dir=None):
     """One instance per rank over `pats` (this rank's shard), reduce group over the ranks; returns the measurements."""
     S, C, P = w["states"], site.getCategoryCount(), pats.patternCount
     scaling = bool(w.get("scaling"))
@@ -478,6 +506,8 @@ def measure_single_partition(D, lib, beagle, w, tree, pats, model, site, steps, 
     # resident eigen system for the asynchronous loop: slot 0 holds it (issue_sync above used parity 0)
     res["blocks"] = timed_blocks(D, stream, step_async, steps, warmup)
     res["joint"] = float(dres.cpu()[0])
+    if dump_dir and D.rank == 0:
+        dump_outputs(dump_dir, inst, ev, S, C, P, (steps - 1) & 1, res["joint"])
     if kernel_timing:
         # kernel classes timed live on the engine's stream, in a block of their own (event pairs around every launch)
         D.bracket()
@@ -487,8 +517,8 @@ def measure_single_partition(D, lib, beagle, w, tree, pats, model, site, steps, 
         D.bracket()
         res["kernels"] = [inst.getKernelTiming(c) for c in range(3)]
         inst.setKernelTiming(False)
-    res["e2e"] = timed_e2e(D, step_e2e, e2e_steps or max(steps, 100))
-    res["e2e"]["c_abi_replay"] = full_evaluations_from_c(inst, ev, min(e2e_steps or max(steps, 100), 400)) if D.world == 1 else None
+    res["e2e"] = timed_e2e(D, step_e2e, steps)
+    res["e2e"]["c_abi_replay"] = full_evaluations_from_c(inst, ev, steps) if D.world == 1 else None
     return res
 
 
@@ -641,10 +671,9 @@ def strong_makona(D, lib, beagle, steps, warmup):
     w, tree, pats, model, site = build_workload("makona_like_1610x6k", 0, {})
     w = dict(w, scaling=True)                      # deep tree: evaluated rescaled, the way BEAST does after its first underflow
     shard = pats.subSet(D.rank, D.world) if D.world > 1 else pats
-    r = measure_single_partition(D, lib, beagle, w, tree, shard, model, site, steps, warmup, kernel_timing=True,
-                                 e2e_steps=max(steps, 100))
+    r = measure_single_partition(D, lib, beagle, w, tree, shard, model, site, steps, warmup, kernel_timing=True)
     b = r["blocks"]
-    ms = b["block_ms_p50"] / steps
+    ms = b["block_ms_p50"]
     k_ms = r["kernels"][0][0] / steps
     r["inst"].finalize()
     return {"workload": "makona_like_1610x6k split into %d contiguous pattern blocks (Patterns.java:142-169), rescaled" % D.world,
@@ -657,7 +686,7 @@ def strong_makona(D, lib, beagle, steps, warmup):
 def flu8_partitions():
     tree = em.Tree.coalescent(2000, 0.05, 5)
     parts, models, sites = [], [], []
-    cache = os.path.join(os.environ.get("B200_BENCH_CACHE", "/tmp/b200_bench_cache"), "flu8_2000.npz")
+    cache = os.path.join(BENCH_CACHE, "flu8_2000.npz")
     z = np.load(cache, allow_pickle=False) if os.path.exists(cache) else None
     for k, ns in enumerate(FLU8_SITES):
         rng = np.random.default_rng(10 + k)
@@ -734,8 +763,8 @@ def strong_flu8(D, lib, beagle, steps, warmup):
     step_async(0)
     stream = external_stream(D, strm)
     blocks = timed_blocks(D, stream, step_async, steps, warmup)
-    e2e = timed_e2e(D, step_e2e, max(steps, 50))
-    ms = blocks["block_ms_p50"] / steps
+    e2e = timed_e2e(D, step_e2e, steps)
+    ms = blocks["block_ms_p50"]
     b.finalize()
     return {"workload": "flu8_like: 8 partitions (%s sites), 2000 taxa, GTR+G4 each, partition k on GPU k mod %d, one "
                         "*ByPartition instance per GPU" % ("/".join(map(str, FLU8_SITES)), D.world),
@@ -743,13 +772,6 @@ def strong_flu8(D, lib, beagle, steps, warmup):
             "e2e_joint_evals_per_s": 1.0 / e2e["median_s"], "e2e_ms_per_step": e2e["median_ms"],
             "repeats": blocks["repeats"], "block_ms_p10": blocks["block_ms_p10"], "block_ms_p90": blocks["block_ms_p90"],
             "logL": e2e["logL"], "steps": steps}
-
-
-def load_json(path):
-    try:
-        return json.load(open(path))
-    except (OSError, ValueError):
-        return None
 
 
 def main():
@@ -766,6 +788,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the strong-scaling / incremental / cold-plan sections")
     ap.add_argument("--cpu-budget", type=float, default=12.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -798,8 +821,11 @@ def main():
     sampler = ClockSampler(D.local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
-    r = measure_single_partition(D, lib, beagle, w, tree, pats, model, site, args.steps, args.warmup)
-    clocks = sampler.stop() if sampler else None
+    try:
+        r = measure_single_partition(D, lib, beagle, w, tree, pats, model, site, args.steps, args.warmup,
+                                     dump_dir=args.dump_outputs)
+    finally:
+        clocks = sampler.stop() if sampler else None
     ev, inst, S, C, P, out = r["ev"], r["inst"], r["S"], r["C"], r["P"], r["out"]
     scaling = bool(w.get("scaling"))
 
@@ -824,37 +850,26 @@ def main():
 
     blocks = r["blocks"]
     dev_ms = blocks["block_ms_p50"]
-    value = world * args.steps / (dev_ms * 1e-3)
+    value = world * 1e3 / dev_ms
     byt, flo = ev.algorithmic(S, C, P)
     (k_ms, k_n), (m_ms, m_n), (r_ms, r_n) = r["kernels"]
     k_avg_ms = k_ms / args.steps
-    peaks = load_json(os.path.join(ROOT, "MEASURED_PEAKS.json"))
-    fp64 = load_json(os.path.join(ROOT, "profiles", "r02_fp64_peaks.json"))
-    traffic_tab = load_json(os.path.join(ROOT, "profiles", "r02_traffic.json")) or {}
-    tj = None if custom else traffic_tab.get(args.workload)
-    traffic = (tj["dram_bytes_read_per_step"] + tj["dram_bytes_write_per_step"]) if tj else None
     if S > 20:
         # dense contraction: the FP64 tensor pipe (mma.sync m8n8k4, SASS DMMA) is the roofline (10.2 flop/B at S = 61)
-        peak = fp64["dmma_m8n8k4_tflops"] if fp64 else 37.0
-        peak_src = "profiles/r02_fp64_peaks.json dmma_m8n8k4_tflops (tools/fp64_peaks.cu, measured on this pool's B200)" \
-            if fp64 else "fallback 37 TFLOP/s"
+        peak = H100_FP64_TENSOR_TFLOPS
+        peak_src = "H100 SXM data sheet, FP64 tensor core dense (not a measured peak)"
         achieved = flo / (k_avg_ms * 1e-3) / 1e12
         roof = {"bound": "fp64", "kernel": "k_walk_mma (updatePartials on the fp64 tensor pipe, DMMA m8n8k4)",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak}
     else:
-        peak = peaks["hbm_gbs"] if peaks else 6650.0
-        peak_src = "MEASURED_PEAKS.json hbm_gbs (copy, burst)" if peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
+        peak = H100_HBM_GBS
+        peak_src = "H100 SXM data sheet, HBM3 bandwidth (not a measured peak)"
         achieved = byt / (k_avg_ms * 1e-3) / 1e9
         roof = {"bound": "hbm", "kernel": ("k_walk4e (updatePartials in eigen form, whole op list in a few launches)"
                                            if S <= 4 else "k_walk_mma (updatePartials on the fp64 tensor pipe)"),
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak}
-    hbm_peak = peaks["hbm_gbs"] if peaks else 6650.0
     roof.update({
-        "traffic": traffic, "traffic_source": tj["source"] if tj else None, "peak_source": peak_src,
-        # DRAM-side view of the same launches: measured bytes (ncu) over the live time.  The algorithmic bytes count every
-        # child read, of which those forwarded in registers or served by L2 never reach HBM; dram_frac cannot exceed 1.
-        "dram_achieved": (traffic / (k_avg_ms * 1e-3) / 1e9) if traffic else None,
-        "dram_frac": (traffic / (k_avg_ms * 1e-3) / 1e9 / hbm_peak) if traffic else None,
+        "peak_source": peak_src,
         "algorithmic_bytes_per_step": byt, "algorithmic_flops_per_step": flo,
         "gflops": flo / (k_avg_ms * 1e-3) / 1e9, "hbm_gbs_algorithmic": byt / (k_avg_ms * 1e-3) / 1e9,
         "partials_ms_per_step": k_avg_ms, "launches_per_step": k_n / args.steps,
@@ -865,11 +880,11 @@ def main():
     line = dict(meta_base)
     line.update({
         "value": value, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
-        "ms_per_step": dev_ms / args.steps, "wall_ms_per_step": blocks["wall_ms_per_step"],
+        "ms_per_step": dev_ms, "wall_ms_per_step": blocks["wall_ms_per_step"], "timed_ms": blocks["total_ms"],
         "repeats": blocks["repeats"], "block_ms_p10": blocks["block_ms_p10"], "block_ms_p50": blocks["block_ms_p50"],
         "block_ms_p90": blocks["block_ms_p90"],
-        "statistic": "median over `repeats` blocks of `steps` steps, each block = max over ranks of its CUDA-event time",
-        "vs_baseline": None, "logL": r["joint"], "joint_evals_per_s": args.steps / (dev_ms * 1e-3),
+        "statistic": "median over the `steps` timed steps, each step = max over ranks of its CUDA-event time",
+        "vs_baseline": None, "logL": r["joint"], "joint_evals_per_s": 1e3 / dev_ms,
         "roofline": roof,
         "e2e": {"value": world / e2e["median_s"], "unit": "evals/s", "ms_per_step": e2e["median_ms"],
                 "h2d_bytes_per_step": ev.h2d_bytes(S, C), "d2h_bytes_per_step": 8, "logL": e2e["logL"],
@@ -884,7 +899,7 @@ def main():
     if not args.no_cpu_baseline:
         from beast_mcmc_b200 import build
         build.build_oracle()
-        cores = os.cpu_count() or 1
+        cores = usable_cores()
         evc = Evaluation(tree, pats, model, site, "POST_ORDER", scaling=scaling)
         threads, tried = cpu_pick_threads(evc, S, C, P, cores)
         times, cval = cpu_time_evaluations(evc, S, C, P, threads, 5, args.cpu_budget)

@@ -1,5 +1,5 @@
 /*
- * libhmsbeagle_b200.h -- the drop-in boundary of the B200 tree-likelihood engine.
+ * libhmsbeagle_b200.h -- the drop-in boundary of the H100 tree-likelihood engine.
  *
  * BEAST (beast-dev/beast-mcmc) reaches its likelihood arithmetic through
  *     beagle.Beagle (interface, lib/beagle.jar)  ->  beagle.BeagleJNIWrapper (47 natives)
@@ -154,7 +154,7 @@ typedef struct {
 BEAGLE_DLLEXPORT const char* beagleGetVersion(void);
 BEAGLE_DLLEXPORT const char* beagleGetCitation(void);
 /* native getResourceList(): 0 = host fallback (reported, not implemented: creating on it yields
- * BEAGLE_ERROR_NO_RESOURCE), 1..N = the visible B200s ("0 == CPU", BDLD:71-73,275-281). */
+ * BEAGLE_ERROR_NO_RESOURCE), 1..N = the visible GPUs ("0 == CPU", BDLD:71-73,275-281). */
 BEAGLE_DLLEXPORT BeagleResourceList* beagleGetResourceList(void);
 /* native getBenchmarkedResourceList (BDLD:413-426, -beagle_auto) */
 BEAGLE_DLLEXPORT BeagleBenchmarkedResourceList* beagleGetBenchmarkedResourceList(
@@ -332,7 +332,7 @@ BEAGLE_DLLEXPORT int b200RootLogLikelihoodDevice(int instance, int bufferIndex, 
                                                  void** outDevicePointer, void** outStream);
 
 /* ---- multi-GPU (SURVEY.md 8e) -----------------------------------------------------------------------------------
- * Mode B, one instance over several GPUs: beagleGetResourceList() ends with a resource "B200 x N (pattern-sharded)" on
+ * Mode B, one instance over several GPUs: beagleGetResourceList() ends with a resource "GPU x N (pattern-sharded)" on
  * boxes with >= 2 GPUs; an instance created on it splits its patterns into contiguous blocks (the rule of BEAST's own
  * -beagle_instances split, src/dr/evolution/alignment/Patterns.java:142-169) over the GPUs and behaves like any other
  * instance -- beagleCalculateRootLogLikelihoods returns the joint value (CompoundLikelihood.java:214-219 sums the same

@@ -75,13 +75,20 @@ static void* worker_main(void* arg) {
     const int tid = w->tid;
     free(w);
     /* one worker per hardware thread, pinned: the pattern block a thread owns stays on the NUMA node that first touched
-     * it (the partials are first written inside the walk, by the owning thread) */
-    const long ncpu = sysconf(_SC_NPROCESSORS_ONLN);
-    if (ncpu > 0 && o->threads <= ncpu) {
-        cpu_set_t set;
-        CPU_ZERO(&set);
-        CPU_SET((int)(tid % ncpu), &set);
-        pthread_setaffinity_np(pthread_self(), sizeof set, &set);
+     * it (the partials are first written inside the walk, by the owning thread).  Pin within the CPUs this process may
+     * run on: pinning to CPU ids outside that set stacks spinning workers on the same few cores, and every spin barrier
+     * then waits for descheduled threads */
+    cpu_set_t allowed;
+    if (sched_getaffinity(0, sizeof allowed, &allowed) == 0 && o->threads <= CPU_COUNT(&allowed)) {
+        int k = tid % CPU_COUNT(&allowed);
+        for (int c = 0; c < CPU_SETSIZE; ++c) {
+            if (!CPU_ISSET(c, &allowed) || k-- > 0) continue;
+            cpu_set_t set;
+            CPU_ZERO(&set);
+            CPU_SET(c, &set);
+            pthread_setaffinity_np(pthread_self(), sizeof set, &set);
+            break;
+        }
     }
     int s0 = 0, s1 = 0;
     for (;;) {

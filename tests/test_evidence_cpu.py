@@ -20,7 +20,7 @@ def _line(name):
 
 
 def test_sass_excerpts_were_taken_from_this_tree():
-    path = os.path.join(P, "r02_sass_excerpts.txt")
+    path = os.path.join(P, "h100_sass_excerpts.txt")
     if not os.path.exists(path):
         pytest.skip("no SASS excerpts collected yet")
     m = re.search(r"library source hash (\w+)", open(path).read())
@@ -34,7 +34,7 @@ def test_sass_excerpts_were_taken_from_this_tree():
         assert rows and mnemonic in rows[0], (kernel, mnemonic)
 
 
-@pytest.mark.parametrize("name", ["r02_bench_cfg2.json", "r02_bench_codon.json", "r02_bench_cfg2_steps20.json"])
+@pytest.mark.parametrize("name", ["h100_bench_cfg2.json", "h100_bench_codon.json", "h100_bench_cfg2_steps20.json"])
 def test_bench_line_contract(name):
     d = _line(name)
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
@@ -46,17 +46,18 @@ def test_bench_line_contract(name):
     r = d["roofline"]
     assert r["bound"] == ("fp64" if d["config"]["states"] > 20 else "hbm")
     assert abs(r["frac"] - r["achieved"] / r["peak"]) <= 1e-9 * max(1.0, r["frac"])
-    assert d["warmup"] >= 3 and d["repeats"] >= 25 and d["gpu_launches"] > 0
+    assert d["warmup"] >= 3 and d["repeats"] == d["steps"] >= 20 and d["gpu_launches"] > 0
+    assert d["clocks"]["gpu"] and "H100" in d["clocks"]["gpu"] and d["clocks"]["power_limit_w"] > 0
     e = d["e2e"]
     assert e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] == 8 and e["value"] != d["value"]
     assert not set(d["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
-    # value = steps / (median block) up to the max-over-ranks bookkeeping
+    # value = 1 / (median step) up to the max-over-ranks bookkeeping
     assert abs(d["value"] - d["n_gpus"] * 1e3 / d["ms_per_step"]) <= 1e-6 * d["value"]
 
 
 def test_reference_arm_line_contract():
-    d = _line("r02_bench_cfg2_reference.json")
+    d = _line("h100_bench_cfg2_reference.json")
     assert d["impl"] == "reference" and d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] >= 1
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0 and d["e2e"]["value"] == d["value"]
-    g = _line("r02_bench_cfg2.json")
+    g = _line("h100_bench_cfg2.json")
     assert d["metric"] == g["metric"] and d["unit"] == g["unit"] and d["config"]["workload"] == g["config"]["workload"]

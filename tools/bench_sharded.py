@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Mode B (SURVEY.md 8e): ONE BEAGLE instance whose patterns the engine shards over g GPUs of this process (csrc/multi.cu)
--- what an unmodified BEAST run sees when it names the "B200 x N (pattern-sharded)" resource.  Times full evaluations
+-- what an unmodified BEAST run sees when it names the "GPU x N (pattern-sharded)" resource.  Times full evaluations
 through the synchronous reference-facing calls (host buffers in, joint log-likelihood out) for g = 1, 2, 4, 8 (as many as
 the box has) on one alignment, and checks the value against the single-GPU instance.  Prints one JSON line."""
 import ctypes as C

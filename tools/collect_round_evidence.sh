@@ -1,7 +1,7 @@
 #!/bin/bash
-# One GPU-box pass that regenerates the raw material under profiles/ for a round:  bash tools/collect_round_evidence.sh r02
+# One GPU-box pass that regenerates the raw material under profiles/ for a round:  bash tools/collect_round_evidence.sh h100
 # (everything lands in gpurun_out/; tools/summarise_round_evidence.py turns it into the committed summaries here)
-R=${1:-r02}
+R=${1:-h100}
 mkdir -p gpurun_out
 ./tools/bin/fp64_peaks > gpurun_out/${R}_fp64_peaks.json 2> gpurun_out/${R}_fp64_peaks.err; cat gpurun_out/${R}_fp64_peaks.json
 python -m pytest tests -m gpu -q 2>&1 | tail -3 > gpurun_out/${R}_gpu_tests.txt; cat gpurun_out/${R}_gpu_tests.txt

@@ -2,7 +2,7 @@
 //   * register-resident DFMA chains (the CUDA-core fp64 pipe the 4-state kernels use)
 //   * mma.sync.aligned.m8n8k4.f64 chains (SASS DMMA.8x8x4, the fp64 tensor path of k_walk_mma)
 //   * a pure streaming write and a read+write copy (the HBM floor of the 4-state walk is its destination writes)
-// Prints ONE JSON line.  Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peaks tools/fp64_peaks.cu
+// Prints ONE JSON line.  Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peaks tools/fp64_peaks.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -44,19 +44,21 @@ __global__ void __launch_bounds__(256) k_dmma(double* out, int iters, double a, 
     if (s == 12345.678) out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
-// 256-bit accesses (st.global.v4.f64 / ld.global.v4.f64, SASS STG.E.ENL2.256 / LDG.E.ENL2.256: what the walk kernels issue)
+// one 32-byte cell per thread as two 128-bit accesses (sm_90 has no 256-bit global access): what the walk kernels issue
 __global__ void __launch_bounds__(256) k_fill(double4* dst, size_t n4, double v) {
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
-        asm volatile("st.global.v4.f64 [%0], {%1,%1,%1,%1};" :: "l"(dst + i), "d"(v) : "memory");
+        asm volatile("st.global.v2.f64 [%0], {%1,%1};\n\tst.global.v2.f64 [%0+16], {%1,%1};" :: "l"(dst + i), "d"(v) : "memory");
 }
 
 __global__ void __launch_bounds__(256) k_copy(double4* dst, const double4* src, size_t n4) {
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
         double a, b, c, d;
-        asm volatile("ld.global.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(src + i) : "memory");
-        asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};" :: "l"(dst + i), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
+        asm volatile("ld.global.v2.f64 {%0,%1}, [%4];\n\tld.global.v2.f64 {%2,%3}, [%4+16];"
+                     : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(src + i) : "memory");
+        asm volatile("st.global.v2.f64 [%0], {%1,%2};\n\tst.global.v2.f64 [%0+16], {%3,%4};"
+                     :: "l"(dst + i), "d"(a), "d"(b), "d"(c), "d"(d) : "memory");
     }
 }
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Turn the raw material a GPU-box pass left in gpurun_out/ (tools/collect_round_evidence.sh) into the committed summaries
-under profiles/:  python tools/summarise_round_evidence.py r02
+under profiles/:  python tools/summarise_round_evidence.py h100
 
   <R>_traffic.json     DRAM bytes per step of the updatePartials launches, per workload (ncu dram__bytes_{read,write}.sum)
   <R>_ncu_raw.txt      selected metrics of the --set full captures (tools/ncu_summary.py)
@@ -16,7 +16,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-R = sys.argv[1] if len(sys.argv) > 1 else "r02"
+R = sys.argv[1] if len(sys.argv) > 1 else "h100"
 G = os.path.join(ROOT, "gpurun_out")
 P = os.path.join(ROOT, "profiles")
 os.makedirs(P, exist_ok=True)
@@ -101,15 +101,15 @@ def sass_excerpts():
     with open(os.path.join(P, f"{R}_sass_excerpts.txt"), "w") as f:
         f.write("# SASS mnemonic counts per kernel of the shipped libhmsbeagle.so (cuobjdump -sass; static instruction counts)\n")
         f.write("# DMMA = mma.sync m8n8k4 f64 (fp64 tensor pipe); UBLKCP/SYNCS = cp.async.bulk + mbarrier (TMA engine);\n")
-        f.write("# LDGSTS = cp.async; LDG/STG.E.ENL2.256 = 256-bit global accesses; LDCU/R2UR + DFMA = constant-bank operands through\n")
-        f.write("# uniform registers; no UTC*MMA / LDTM / UTMALDG: tcgen05 has no fp64 kind (SURVEY.md 7, hard part 2)\n")
+        f.write("# LDGSTS = cp.async; LDCU/R2UR + DFMA = constant-bank operands through\n")
+        f.write("# uniform registers; no HGMMA: wgmma has no fp64 kind\n")
         source_hash = subprocess.run([sys.executable, "-c", "import sys; sys.path.insert(0, %r); import beast_mcmc_b200; "
                                       "from beast_mcmc_b200 import build; print(build.verify_engine())" % ROOT],
                                      capture_output=True, text=True).stdout.strip()
         f.write(f"# library source hash {source_hash}\n")
         for k in keep:
             if k in per:
-                f.write(f"{k}: " + ", ".join(f"{op} {n}" for op, n in sorted(per[k].items())) + "\n")
+                f.write((f"{k}: " + ", ".join(f"{op} {n}" for op, n in sorted(per[k].items()))).rstrip() + "\n")
         total = {}
         for d in per.values():
             for op, n in d.items():
