@@ -159,6 +159,7 @@ void destroyInstance(Instance* in) {
     cudaFree(in->partialsBase); cudaFree(in->states8Base); cudaFree(in->states32Base);
     for (CachedPlan& cp : in->planCache) { cp.dropGraph(); cudaFree(cp.dBlock); }
     cudaFree(in->dEigen); cudaFree(in->dMat); cudaFree(in->dEvec); cudaFree(in->dIncSums); cudaFree(in->dIncCounter);
+    cudaFree(in->dRecipe);
     if (in->hMapped) cudaFreeHost(in->hMapped); cudaFree(in->dRates); cudaFree(in->dWeights);
     cudaFree(in->dFreqs); cudaFree(in->dScale); cudaFree(in->dPatternWeights);
     cudaFree(in->dPatternPartitions); cudaFree(in->dSite); cudaFree(in->dBlockSums); cudaFree(in->dOut);
@@ -430,20 +431,27 @@ void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, int fixedT
 }
 
 // launch the phases of a prepared plan (device-resident op records + subtree table)
-// eigenSlot >= 0: the 4-state list runs in eigen form (walk4e.cu) with that slot's V / V^-1; aligned: no pattern windows
+// eigenSlot >= 0: the 4-state list runs in eigen form (walk4e.cu) with that slot's V / V^-1; aligned: no pattern windows;
+// nSnap: virtual cherries the list produces (their recipes are snapshot first); virt: the records name virtual cherries
 cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const std::vector<int>& phaseStart,
                        const std::vector<int>& phaseDepth, bool fourPath, int maxWindow, bool preOrder, int eigenSlot = -1,
-                       bool aligned = false) {
+                       bool aligned = false, const void* dSnap = nullptr, int nSnap = 0, const void* dVirtTips = nullptr) {
+    const bool virt = dVirtTips != nullptr;
     cudaError_t e = cudaSuccess;
+    if (nSnap > 0) {
+        TimedScope ts(in, T_PARTIALS);
+        e = launchCherrySnapshot(in, static_cast<const int4*>(dSnap), nSnap);
+    }
     for (size_t ph = 0; ph + 1 < phaseStart.size() && e == cudaSuccess; ++ph) {
         const int s0 = phaseStart[ph], s1 = phaseStart[ph + 1];
         if (s1 <= s0) continue;
         TimedScope ts(in, T_PARTIALS);
         if (fourPath && eigenSlot >= 0 && !preOrder && (ph >= phaseDepth.size() || phaseDepth[ph] == 0)) {
             e = launchWalk4E(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
-                             aligned, in->hEigen.data() + (size_t)eigenSlot * 36);
+                             aligned, in->hEigen.data() + (size_t)eigenSlot * 36, static_cast<const int4*>(dVirtTips));
             continue;
         }
+        if (virt) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
         e = fourPath ? launchWalk4(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0,
                                    ph < phaseDepth.size() ? phaseDepth[ph] : 0, maxWindow, preOrder)
                      : launchWalkGeneric(in, static_cast<const DevOp*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0,
@@ -468,6 +476,59 @@ cudaError_t accumulateInList(Instance* in, const std::vector<CumGroup>& groups) 
 // per-node scale buffers written by a list hold raw factors (logs under SCALERS_LOG)
 void noteScaleWrites(Instance* in, const std::vector<HostOp>& hops) {
     for (const HostOp& o : hops) if (o.sw >= 0) in->scaleIsLog[o.sw] = in->logScalers ? 1 : 0;
+}
+
+// ---- virtual cherries (walk4e.cu) ----------------------------------------------------------------------------------
+// A tip x tip op without rescaling in a list the eigen-form walk runs on k_walk4p is not run: its consumers recompute
+// colA ⊙ colB from a recipe (the two P blocks, snapshot when the list runs) and the two tips' state bytes.  Its partials
+// are written only when something else reads the buffer, through storeCherries -- the one place that happens.
+
+// every reader of stored partials other than k_walk4pv calls this with the buffers it is about to read: virtual cherries
+// among them get their partials written (they stay virtual-readable: the recipe is still valid)
+cudaError_t storeCherries(Instance* in, const int* bufs, int count) {
+    if (in->cherryTip1.empty()) return cudaSuccess;
+    std::vector<int4> items;
+    for (int k = 0; k < count; ++k) {
+        const int b = bufs[k];
+        if (!validRange(b, in->nBuffers) || in->cherryTip1[b] < 0 || in->cherryStored[b]) continue;
+        items.push_back(make_int4(in->slotOf[b], b, in->cherryTip1[b], in->cherryTip2[b]));
+        in->cherryStored[b] = 1;
+    }
+    if (items.empty()) return cudaSuccess;
+    const int4* dItems = static_cast<const int4*>(stage(in, items.data(), sizeof(int4) * items.size()));
+    cudaError_t e = cudaErrorMemoryAllocation;
+    if (dItems != nullptr) {
+        TimedScope ts(in, T_PARTIALS);
+        e = launchCherryStore(in, dItems, (int)items.size());
+    }
+    if (e != cudaSuccess) for (const int4& it : items) in->cherryStored[it.y] = 0;
+    return e;
+}
+
+// children a list reads from outside itself as stored partials
+cudaError_t storeExternal(Instance* in, const std::vector<CherryRef>& external) {
+    std::vector<int> bufs;
+    for (const CherryRef& x : external) if (x.tip1 < 0) bufs.push_back(x.buf);
+    return storeCherries(in, bufs.data(), (int)bufs.size());
+}
+
+// tip t is about to change: the cherries computed from it get their partials written and are plain partials from now on
+cudaError_t settleCherriesOf(Instance* in, int t) {
+    std::vector<int> deps;
+    for (int b = 0; b < (int)in->cherryTip1.size(); ++b)
+        if (in->cherryTip1[b] >= 0 && (in->cherryTip1[b] == t || in->cherryTip2[b] == t)) deps.push_back(b);
+    const cudaError_t e = storeCherries(in, deps.data(), (int)deps.size());
+    if (e == cudaSuccess) for (int b : deps) in->cherryTip1[b] = -1;
+    return e;
+}
+
+// a list ran: its destinations hold real partials, except the virtual cherries it produced
+void noteCherryWrites(Instance* in, const std::vector<HostOp>& hops, const std::vector<CherryRef>& cherries) {
+    if (in->cherryTip1.empty()) return;
+    for (const HostOp& o : hops) in->cherryTip1[o.dest] = -1;
+    for (const CherryRef& c : cherries) {
+        in->cherryTip1[c.buf] = c.tip1; in->cherryTip2[c.buf] = c.tip2; in->cherryStored[c.buf] = 0;
+    }
 }
 
 // validation (no side effects) of an operation list, then lazy allocation / kind changes of its destinations
@@ -526,10 +587,19 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             if (cp.dBlock == nullptr || cp.n != n || cp.byPartition != byPartition || cp.epoch != in->bufferEpoch ||
                 memcmp(cp.key.data(), hops.data(), sizeof(HostOp) * (size_t)n) != 0)
                 continue;
+            const int eigenSlot = cp.fourPath ? eigenFormSlot(in, hops) : -1;
+            // records that name virtual cherries need the eigen form, and an outside child read as a cherry must still be it
+            bool stale = cp.readsVirtual && eigenSlot < 0;
+            for (const CherryRef& x : cp.external)
+                stale = stale || (x.tip1 >= 0 && (in->cherryTip1[x.buf] != x.tip1 || in->cherryTip2[x.buf] != x.tip2));
+            if (stale) { cp.dropGraph(); cp.n = -1; continue; }
+            CUDA_OK(storeExternal(in, cp.external));
             cp.lastUse = ++in->planClock;
             cp.hits++;
-            const int eigenSlot = cp.fourPath ? eigenFormSlot(in, hops) : -1;
             const unsigned eigenGenNow = eigenSlot >= 0 ? in->eigenGen[eigenSlot] : 0u;
+            const void* dSnap = static_cast<char*>(cp.dBlock) + cp.snapOffset;
+            const int nSnap = (int)cp.cherries.size();
+            const void* dTips = cp.readsVirtual ? static_cast<char*>(cp.dBlock) + cp.tipsOffset : nullptr;
             // a captured graph carries the kernel choice and V / V^-1 by value: stale once the eigen system moved on
             if (cp.graphExec != nullptr && (cp.graphEigen != eigenSlot || cp.graphEigenGen != eigenGenNow)) {
                 // same kernels, new V / V^-1 (a substitution-model move): patch the captured launches in place
@@ -545,7 +615,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             }
             // A plan that keeps coming back and needs several dependent launches is replayed as ONE graph launch:
             // on small alignments the host-side launch cost, not the kernels, sets the pace.
-            int launches = 0;
+            int launches = nSnap > 0;
             for (size_t ph = 0; ph + 1 < cp.phaseStart.size(); ++ph) launches += cp.phaseStart[ph + 1] > cp.phaseStart[ph];
             // (in-list cumulative scaling stages its index lists per call: those plans keep the plain launches)
             if (in->useGraphs && launches >= 2 && cp.cumGroups.empty()) {
@@ -553,7 +623,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                     cudaStreamBeginCapture(in->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
                     const cudaError_t e1 = launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart,
                                                       cp.phaseDepth, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
-                                                      !cp.byPartition);
+                                                      !cp.byPartition, dSnap, nSnap, dTips);
                     cp.graphEigen = eigenSlot;
                     cp.graphEigenGen = eigenGenNow;
                     cudaGraph_t g = nullptr;
@@ -579,19 +649,25 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                         }
                         if (cp.graphKernelNodes.empty()) cp.graphAllEigen = false;
                     }
+                    if (getenv("B200_BEAGLE_DEBUG"))
+                        fprintf(stderr, "[b200-beagle] graph %s: %d launches\n", cp.graphExec ? "captured" : "capture failed",
+                                launches);
                     cudaGetLastError();
                 }
                 if (cp.graphExec != nullptr) {
                     TimedScope ts(in, T_PARTIALS, launches);
                     CUDA_OK(cudaGraphLaunch(cp.graphExec, in->stream));
                     noteScaleWrites(in, hops);
+                    noteCherryWrites(in, hops, cp.cherries);
                     return BEAGLE_SUCCESS;
                 }
             }
             CUDA_OK(launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart, cp.phaseDepth,
-                               cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition));
+                               cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap,
+                               dTips));
             CUDA_OK(accumulateInList(in, cp.cumGroups));
             noteScaleWrites(in, hops);
+            noteCherryWrites(in, hops, cp.cherries);
             return BEAGLE_SUCCESS;
         }
     }
@@ -600,26 +676,101 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         if (rcPrepare != BEAGLE_SUCCESS) return rcPrepare;
     }
     const bool fourState = in->matCP > 0;
+    const bool preOrder = hops[0].kind == 1;
+    const int eigenSlot = fourState ? eigenFormSlot(in, hops) : -1;
+    std::vector<char> written(in->nBuffers, 0);
+    std::vector<int> firstWrite(in->nBuffers, n);
+    for (int k = n - 1; k >= 0; --k) { written[hops[k].dest] = 1; firstWrite[hops[k].dest] = k; }
+    // ---- virtual cherries: the ops that are not run (each tip x tip op without rescaling whose destination this list
+    // writes once and reads only afterwards), and whether any op record names a virtual child
+    std::vector<CherryRef> cherries;
+    std::vector<int4> snap;
+    std::vector<HostOp> kept;
+    bool readsVirtual = false;
+    if (!in->cherryTip1.empty() && !byPartition && !preOrder && eigenSlot >= 0 && !in->stackTail) {
+        std::vector<int> writes(in->nBuffers, 0), firstRead(in->nBuffers, n);
+        for (int k = 0; k < n; ++k) {
+            writes[hops[k].dest]++;
+            firstRead[hops[k].c1] = std::min(firstRead[hops[k].c1], k);
+            firstRead[hops[k].c2] = std::min(firstRead[hops[k].c2], k);
+        }
+        for (int k = 0; k < n; ++k) {
+            const HostOp& o = hops[k];
+            if (in->states8[o.c1] != nullptr && in->states8[o.c2] != nullptr && o.sw == BEAGLE_OP_NONE &&
+                o.sr == BEAGLE_OP_NONE && o.cum == BEAGLE_OP_NONE && writes[o.dest] == 1 && firstRead[o.dest] > k) {
+                cherries.push_back(CherryRef{o.dest, o.c1, o.c2});
+                snap.push_back(make_int4(o.dest, o.m1, o.m2, 0));
+            } else {
+                kept.push_back(o);
+            }
+        }
+        if (kept.empty()) { cherries.clear(); snap.clear(); }       // nothing would run: keep the list as it is
+        readsVirtual = !cherries.empty();
+        for (const HostOp& o : hops)
+            for (int c : {o.c1, o.c2})
+                readsVirtual = readsVirtual || (!written[c] && in->states32[c] == nullptr && in->cherryTip1[c] >= 0);
+    }
     Plan plan;
     int maxWindow = in->Ppad;
+    // patterns one warp owns: FMA kernel (32/CP)*R, tensor kernels 8*R resp. 16
+    const int patsPerWarp = !fourState ? 16 : (in->walkVariant == 2 ? 8 * in->tensorR : (32 / in->matCP) * in->walkR);
+    const int warpsPerSM = fourState ? 32 : 12;      // resident warps the kernel family can hold per SM
+    auto wantSubsFor = [&](int window) {
+        const int warpsPerSub = std::max(1, (window + patsPerWarp - 1) / patsPerWarp);
+        // enough (subtree x tile) walks to fill every SM, oversubscribed for balance
+        // oversubscription for balance: 2x where a subtree is only a few warps wide (small alignments), 1x where every
+        // subtree already spreads over dozens of warps -- longer walks forward more results through registers
+        // (measured: cfg 2 +3 %, codon +5 %, benchmark2 +4 %; benchmark1-sized inputs -1..-3 % if forced to 1)
+        const int over = in->phaseOversub > 0 ? in->phaseOversub : (warpsPerSub >= 32 ? 1 : 2);
+        return std::max(1, over * ((in->smCount * warpsPerSM + warpsPerSub - 1) / warpsPerSub));
+    };
+    if (!byPartition && !preOrder) {
+        planPhases(cherries.empty() ? hops : kept, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(in->Ppad),
+                   in->phaseTmin, in->phaseSmall, plan);
+        // only k_walk4p reads virtual children: if some phase of this plan would run elsewhere, every op runs as usual
+        bool served = true;
+        for (size_t ph = 0; readsVirtual && ph + 1 < plan.phaseStart.size(); ++ph) {
+            const int nSubs = plan.phaseStart[ph + 1] - plan.phaseStart[ph];
+            served = served && (nSubs == 0 || walk4pServes(in, nSubs, in->Ppad));
+        }
+        if (!served) {
+            readsVirtual = false;
+            if (!cherries.empty()) {
+                cherries.clear(); snap.clear(); kept.clear();
+                planPhases(hops, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin,
+                           in->phaseSmall, plan);
+            }
+        }
+        for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
+    }
+    // the ops that run
+    const std::vector<HostOp>& L = cherries.empty() ? hops : kept;
+    const int nL = (int)L.size();
+    // children from outside the list -- read at or before the first op that writes them, which may come later in the list
+    // (such lists run in the caller's order): read as virtual cherries where the records can say so, i.e. when the list
+    // never writes them, else as stored partials
+    std::vector<int> vt1(readsVirtual ? in->nBuffers : 0, -1), vt2(readsVirtual ? in->nBuffers : 0, -1);
+    for (const CherryRef& c : cherries) { vt1[c.buf] = c.tip1; vt2[c.buf] = c.tip2; }
+    std::vector<CherryRef> external;
     {
-        // patterns one warp owns: FMA kernel (32/CP)*R, tensor kernels 8*R resp. 16
-        const int patsPerWarp = !fourState ? 16 : (in->walkVariant == 2 ? 8 * in->tensorR : (32 / in->matCP) * in->walkR);
-        const int warpsPerSM = fourState ? 32 : 12;      // resident warps the kernel family can hold per SM
-        auto wantSubsFor = [&](int window) {
-            const int warpsPerSub = std::max(1, (window + patsPerWarp - 1) / patsPerWarp);
-            // enough (subtree x tile) walks to fill every SM, oversubscribed for balance
-            // oversubscription for balance: 2x where a subtree is only a few warps wide (small alignments), 1x where every
-            // subtree already spreads over dozens of warps -- longer walks forward more results through registers
-            // (measured: cfg 2 +3 %, codon +5 %, benchmark2 +4 %; benchmark1-sized inputs -1..-3 % if forced to 1)
-            const int over = in->phaseOversub > 0 ? in->phaseOversub : (warpsPerSub >= 32 ? 1 : 2);
-            return std::max(1, over * ((in->smCount * warpsPerSM + warpsPerSub - 1) / warpsPerSub));
-        };
+        std::vector<char> seen(in->nBuffers, 0);
+        for (int k = 0; k < n; ++k)
+            for (int c : {hops[k].c1, hops[k].c2}) {
+                if (firstWrite[c] < k || in->states32[c] != nullptr || seen[c]) continue;
+                seen[c] = 1;
+                const bool virt = readsVirtual && !written[c] && in->cherryTip1[c] >= 0;
+                external.push_back(CherryRef{c, virt ? in->cherryTip1[c] : -1, virt ? in->cherryTip2[c] : -1});
+                if (virt) { vt1[c] = in->cherryTip1[c]; vt2[c] = in->cherryTip2[c]; }
+            }
+    }
+    CUDA_OK(storeExternal(in, external));
+    {
         if (!byPartition) {
-            if (hops[0].kind == 1 && in->prePhases) planPreorderPhases(hops, in->nBuffers, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin, in->phaseSmall, plan);
-            else if (hops[0].kind == 1) planLevels(hops, in->nBuffers, plan);
-            else planPhases(hops, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin, in->phaseSmall, plan);
-            for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
+            if (preOrder) {
+                if (in->prePhases) planPreorderPhases(hops, in->nBuffers, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin, in->phaseSmall, plan);
+                else planLevels(hops, in->nBuffers, plan);
+                for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
+            }
         } else {
             // partitions are independent (disjoint pattern windows): plan each one on its own and merge the
             // plans phase by phase; every subtree carries its partition's pattern window
@@ -664,7 +815,6 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     // ---- stack slots (4-state path only): one backward pass finds, for every produced value, the
     // position of its LAST reader inside this list (before the buffer is re-written); the forward
     // pass then parks results in slots and frees each slot at that last read.
-    const bool preOrder = hops[0].kind == 1;
     // The operand stack pays off where a phase is LATENCY-bound (few walks in flight: the tail of a full
     // evaluation, or the short dependent chain of an incremental update): it removes the store -> L2 -> load round
     // trip from every op of the chain.  Throughput-bound phases run without it (shared memory would cap occupancy).
@@ -686,8 +836,8 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) subStack[q] = stackEverywhere || thin;
         }
     }
-    std::vector<int> lastReadOfProd(maxDepth > 0 ? n : 0, -1);
-    std::vector<int> subOfPos(n, 0);
+    std::vector<int> lastReadOfProd(maxDepth > 0 ? nL : 0, -1);
+    std::vector<int> subOfPos(nL, 0);
     for (int sIdx = 0; sIdx < (int)plan.subs.size(); ++sIdx)
         for (int q = plan.subs[sIdx].begin; q < plan.subs[sIdx].end; ++q) subOfPos[q] = sIdx;
     if (maxDepth > 0) {
@@ -697,14 +847,14 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             if (!subStack[sIdx]) continue;
             const Sub& sb = plan.subs[sIdx];
             for (int pos = sb.end - 1; pos >= sb.begin; --pos) {
-                const HostOp& o = hops[order[pos]];
+                const HostOp& o = L[order[pos]];
                 lastReadOfProd[pos] = lastRead[o.dest];
                 lastRead[o.dest] = -1;
                 if (lastRead[o.c1] < 0) lastRead[o.c1] = pos;
                 if (lastRead[o.c2] < 0) lastRead[o.c2] = pos;
             }
             for (int pos = sb.begin; pos < sb.end; ++pos) {      // leave no marks for the next subtree
-                const HostOp& o = hops[order[pos]];
+                const HostOp& o = L[order[pos]];
                 lastRead[o.dest] = lastRead[o.c1] = lastRead[o.c2] = -1;
             }
         }
@@ -715,10 +865,11 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
 
     const bool fourPath = in->matCP > 0;
     std::vector<CumGroup> cumGroups;
-    std::vector<DevOp> dops(fourPath ? 0 : n);
-    std::vector<Op4> ops4(fourPath ? n : 0);
-    for (int pos = 0; pos < n; ++pos) {
-        const HostOp& o = hops[order[pos]];
+    std::vector<DevOp> dops(fourPath ? 0 : nL);
+    std::vector<Op4> ops4(fourPath ? nL : 0);
+    std::vector<int4> virtTips(readsVirtual ? nL : 0);     // k_walk4pv: the tips of each op's virtual children
+    for (int pos = 0; pos < nL; ++pos) {
+        const HostOp& o = L[order[pos]];
         const bool t1 = in->states32[o.c1] != nullptr;
         const bool t2 = in->states32[o.c2] != nullptr;
         int srcSlot1 = -1, srcSlot2 = -1, dstSlot = -1;
@@ -762,21 +913,29 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         const int cum = -1;
         if (fourPath) {
             Op4& d = ops4[pos];
+            // a virtual cherry child: its buffer index (recipe row) and its two tips
+            const bool v1 = readsVirtual && !t1 && vt1[o.c1] >= 0, v2 = readsVirtual && !t2 && vt1[o.c2] >= 0;
             d.dest = in->slotOf[o.dest];
-            d.c1 = t1 ? -(o.c1 + 1) : in->slotOf[o.c1];
-            d.c2 = t2 ? -(o.c2 + 1) : in->slotOf[o.c2];
+            d.c1 = t1 ? -(o.c1 + 1) : v1 ? o.c1 : in->slotOf[o.c1];
+            d.c2 = t2 ? -(o.c2 + 1) : v2 ? o.c2 : in->slotOf[o.c2];
             d.m1 = o.m1; d.m2 = o.m2; d.sw = o.sw; d.sr = o.sr; d.cum = cum;
             d.pBegin = pBegin; d.pEnd = pEnd;
             d.slots = (unsigned)(srcSlot1 & 0xFF) | ((unsigned)(srcSlot2 & 0xFF) << 8) | ((unsigned)(dstSlot & 0xFF) << 16);
-            d.pad_ = o.kind;
+            d.pad_ = o.kind | (v1 ? 4 : 0) | (v2 ? 8 : 0);
             d.pfA = d.pfB = 0; d.pfM1 = d.pfM2 = -1;
+            if (readsVirtual)
+                virtTips[pos] = make_int4(v1 ? vt1[o.c1] : 0, v1 ? vt2[o.c1] : 0, v2 ? vt1[o.c2] : 0, v2 ? vt2[o.c2] : 0);
             // register forwarding: inside one subtree walk a thread re-reads, as a child, exactly the cell it wrote for
             // the previous op -- flag it (bit 1), with that child moved to position 1 (the product commutes exactly)
             if (in->forward && !(maxDepth > 0 && subStack[subOfPos[pos]]) && pos > plan.subs[subOfPos[pos]].begin) {
                 const Op4& pv = ops4[pos - 1];
                 if (pv.pBegin == d.pBegin && pv.pEnd == d.pEnd) {
-                    if (!t1 && d.c1 == pv.dest) d.pad_ |= 2;            // pre-order: pre[parent] is the previous result
-                    else if (!preOrder && !t2 && d.c2 == pv.dest) { std::swap(d.c1, d.c2); std::swap(d.m1, d.m2); d.pad_ |= 2; }
+                    if (!t1 && !v1 && d.c1 == pv.dest) d.pad_ |= 2;     // pre-order: pre[parent] is the previous result
+                    else if (!preOrder && !t2 && !v2 && d.c2 == pv.dest) {
+                        std::swap(d.c1, d.c2); std::swap(d.m1, d.m2);
+                        if (readsVirtual) { int4& t = virtTips[pos]; t = make_int4(t.z, t.w, t.x, t.y); }
+                        d.pad_ = (d.pad_ & ~12) | (v1 ? 8 : 0) | 2;
+                    }
                 }
             }
         } else {
@@ -823,13 +982,13 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             for (int pos = plan.subs[sIdx].begin; pos + 1 < plan.subs[sIdx].end; ++pos) {
                 Op4& d = ops4[pos];
                 const Op4& nx = ops4[pos + 1];
-                auto enc = [&](int child, bool fromRegisters) -> int {
-                    if (fromRegisters) return 0;
+                auto enc = [&](int child, bool fromRegisters, bool virt) -> int {
+                    if (fromRegisters || virt) return 0;
                     if (child < 0) return ((-child - 1) << 1) | 1;
                     return child == d.dest ? 0 : ((child + 1) << 1);
                 };
-                d.pfA = enc(nx.c1, (nx.pad_ & 2) != 0);
-                d.pfB = enc(nx.c2, false);
+                d.pfA = enc(nx.c1, (nx.pad_ & 2) != 0, (nx.pad_ & 4) != 0);
+                d.pfB = enc(nx.c2, false, (nx.pad_ & 8) != 0);
                 if (d.pfA == 0) { d.pfA = d.pfB; d.pfB = 0; }
                 d.pfM1 = nx.m1; d.pfM2 = nx.m2;
             }
@@ -838,31 +997,42 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     if (fourPath && getenv("B200_BEAGLE_DEBUG")) {
         int fwd = 0, internal = 0;
         for (const Op4& d : ops4) { fwd += (d.pad_ & 2) != 0; internal += (d.c1 >= 0) + (d.c2 >= 0); }
-        fprintf(stderr, "[b200-beagle] plan: %d ops, %zu subtrees, %d phases, %d internal children, %d forwarded in registers\n",
-                n, plan.subs.size(), nPhases, internal, fwd);
+        fprintf(stderr, "[b200-beagle] plan: %d ops (%zu virtual cherries), %zu subtrees, %d phases, %d internal children, "
+                "%d forwarded in registers\n", nL, cherries.size(), plan.subs.size(), nPhases, internal, fwd);
     }
-    const void* hostOps = fourPath ? (const void*)ops4.data() : (const void*)dops.data();
-    const size_t opBytes = (fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)n;
+    // one block: [op records | subtree table | snapshot items], each part 256-byte aligned
+    const size_t opBytes = (fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)nL;
     const size_t subBytes = sizeof(Sub) * plan.subs.size();
-    void* dOps = stage(in, hostOps, opBytes);
-    void* dSubs = stage(in, plan.subs.data(), subBytes);
+    const size_t snapBytes = sizeof(int4) * snap.size();
+    const size_t subsOffset = (opBytes + 255) & ~size_t(255);
+    const size_t snapOffset = subsOffset + ((subBytes + 255) & ~size_t(255));
+    const size_t tipsBytes = sizeof(int4) * virtTips.size();
+    const size_t tipsOffset = snapOffset + ((snapBytes + 255) & ~size_t(255));
+    const size_t blockBytes = tipsOffset + tipsBytes;
+    std::vector<char> hBlock(blockBytes, 0);
+    memcpy(hBlock.data(), fourPath ? (const void*)ops4.data() : (const void*)dops.data(), opBytes);
+    memcpy(hBlock.data() + subsOffset, plan.subs.data(), subBytes);
+    if (snapBytes) memcpy(hBlock.data() + snapOffset, snap.data(), snapBytes);
+    if (tipsBytes) memcpy(hBlock.data() + tipsOffset, virtTips.data(), tipsBytes);
+    void* dOps = stage(in, hBlock.data(), blockBytes);
     void* tmp = nullptr;
-    if (dOps == nullptr || dSubs == nullptr) {
+    if (dOps == nullptr) {
         // list larger than the staging ring: one-off allocation
-        CUDA_OK(cudaMalloc(&tmp, opBytes + 256 + subBytes));
+        CUDA_OK(cudaMalloc(&tmp, blockBytes));
         dOps = tmp;
-        dSubs = static_cast<char*>(tmp) + ((opBytes + 255) & ~size_t(255));
-        cudaError_t ce = cudaMemcpyAsync(dOps, hostOps, opBytes, cudaMemcpyHostToDevice, in->stream);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync(dSubs, plan.subs.data(), subBytes, cudaMemcpyHostToDevice, in->stream);
+        cudaError_t ce = cudaMemcpyAsync(dOps, hBlock.data(), blockBytes, cudaMemcpyHostToDevice, in->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(in->stream);
         if (ce != cudaSuccess) { cudaFree(tmp); CUDA_OK(ce); }
     }
+    void* dSubs = static_cast<char*>(dOps) + subsOffset;
     std::vector<int> depths(plan.phaseStart.size(), 0);
     for (size_t ph = 0; ph + 1 < plan.phaseStart.size(); ++ph) depths[ph] = (maxDepth > 0 && ph < phaseDepth.size()) ? phaseDepth[ph] : 0;
-    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, depths, fourPath, maxWindow, preOrder,
-                               fourPath ? eigenFormSlot(in, hops) : -1, !byPartition);
+    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, depths, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
+                               static_cast<char*>(dOps) + snapOffset, (int)snap.size(),
+                               readsVirtual ? static_cast<char*>(dOps) + tipsOffset : nullptr);
     if (e == cudaSuccess) e = accumulateInList(in, cumGroups);
     noteScaleWrites(in, hops);
+    if (e == cudaSuccess) noteCherryWrites(in, hops, cherries);
     if (e == cudaSuccess && tmp == nullptr && in->planCacheSize > 0) {
         // remember the plan: device copy of the records (stream-ordered D2D out of the staging ring)
         if ((int)in->planCache.size() < in->planCacheSize) in->planCache.emplace_back();
@@ -871,22 +1041,21 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             if (cp.dBlock == nullptr || cp.n < 0) { slot = &cp; break; }
             if (slot == nullptr || cp.lastUse < slot->lastUse) slot = &cp;
         }
-        const size_t subsOffset = (opBytes + 255) & ~size_t(255);
-        const size_t need = subsOffset + subBytes;
         slot->dropGraph();
         slot->hits = 0;
         slot->graphFailed = false;
         slot->graphInvalidations = 0;
-        if (slot->capacity < need) {
+        if (slot->capacity < blockBytes) {
             if (slot->dBlock) cudaFree(slot->dBlock);
             slot->dBlock = nullptr; slot->capacity = 0;
-            if (cudaMalloc(&slot->dBlock, need) == cudaSuccess) slot->capacity = need; else cudaGetLastError();
+            if (cudaMalloc(&slot->dBlock, blockBytes) == cudaSuccess) slot->capacity = blockBytes; else cudaGetLastError();
         }
         if (slot->dBlock != nullptr &&
-            cudaMemcpyAsync(slot->dBlock, dOps, opBytes, cudaMemcpyDeviceToDevice, in->stream) == cudaSuccess &&
-            cudaMemcpyAsync(static_cast<char*>(slot->dBlock) + subsOffset, dSubs, subBytes, cudaMemcpyDeviceToDevice, in->stream) == cudaSuccess) {
+            cudaMemcpyAsync(slot->dBlock, dOps, blockBytes, cudaMemcpyDeviceToDevice, in->stream) == cudaSuccess) {
             slot->key = hops; slot->n = n; slot->byPartition = byPartition; slot->epoch = in->bufferEpoch;
-            slot->subsOffset = subsOffset; slot->phaseStart = plan.phaseStart; slot->phaseDepth = depths;
+            slot->subsOffset = subsOffset; slot->snapOffset = snapOffset; slot->tipsOffset = tipsOffset;
+            slot->cherries = cherries; slot->external = external; slot->readsVirtual = readsVirtual;
+            slot->phaseStart = plan.phaseStart; slot->phaseDepth = depths;
             slot->fourPath = fourPath; slot->maxWindow = maxWindow; slot->preOrder = preOrder;
             slot->lastUse = ++in->planClock;
             slot->cumGroups = cumGroups;
@@ -1025,6 +1194,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->eigenWalk = envInt("B200_EIGEN_WALK", 1);
     in->tipMode = envInt("B200_TIP_MODE", 3);
     in->thinTipMode = envInt("B200_THIN_TIP_MODE", in->tipMode);
+    in->virtualCherries = envInt("B200_VIRTUAL_CHERRIES", 1);
     in->walkBlock = 128;
     in->walkVariant = envInt("B200_WALK_VARIANT", 0);
     in->reorder = envInt("B200_REORDER", 1);
@@ -1075,6 +1245,12 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     alloc(&in->dEigen, std::max(1, in->nEigen) * eigenStride);
     alloc(&in->dMat, matElems);
     if (in->matCP > 0) alloc(&in->dEvec, (size_t)in->nMatrices * in->matCP * 4);
+    if (in->matCP > 0 && in->matCP <= 8 && in->virtualCherries) {
+        alloc(&in->dRecipe, (size_t)in->nBuffers * 32 * in->matCP);
+        in->cherryTip1.assign(in->nBuffers, -1);
+        in->cherryTip2.assign(in->nBuffers, -1);
+        in->cherryStored.assign(in->nBuffers, 0);
+    }
     if (in->matCP > 0 && in->matCP <= 8) {
         alloc(&in->dIncSums, (size_t)in->Ppad / 4 + 8);
         alloc(&in->dIncCounter, 4);
@@ -1200,6 +1376,7 @@ int beagleSetTipStates(int instance, int tipIndex, const int* inStates) {
         s8[p] = (uint8_t)s;
     }
     if (tipIndex >= in->tipCount) return BEAGLE_ERROR_OUT_OF_RANGE;
+    CUDA_OK(settleCherriesOf(in, tipIndex));      // cherries computed from the old states keep their values
     in->states32[tipIndex] = in->states32Base + (size_t)tipIndex * in->Ppad;
     in->states8[tipIndex] = in->states8Base + (size_t)tipIndex * in->Ppad;
     CUDA_OK(cudaMemcpyAsync(in->states32[tipIndex], s32.data(), sizeof(int) * in->Ppad, cudaMemcpyHostToDevice, in->stream));
@@ -1224,6 +1401,8 @@ static int setPartialsImpl(Instance* in, int bufferIndex, const double* inPartia
     if (!validRange(bufferIndex, in->nBuffers) || inPartials == nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
     double* dst = ensurePartials(in, bufferIndex);
     if (dst == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
+    CUDA_OK(settleCherriesOf(in, bufferIndex));
+    if (!in->cherryTip1.empty()) in->cherryTip1[bufferIndex] = -1;
     std::vector<double> tmp(in->partialsElems, 0.0);
     for (int c = 0; c < in->C; ++c)
         for (int p = 0; p < in->Ppad; ++p) {
@@ -1261,6 +1440,7 @@ int beagleGetPartials(int instance, int bufferIndex, int scaleIndex, double* out
     if (!validRange(bufferIndex, in->nBuffers) || in->partials[bufferIndex] == nullptr || outPartials == nullptr)
         return BEAGLE_ERROR_OUT_OF_RANGE;
     if (scaleIndex != BEAGLE_OP_NONE && !validRange(scaleIndex, in->nScale)) return BEAGLE_ERROR_OUT_OF_RANGE;
+    CUDA_OK(storeCherries(in, &bufferIndex, 1));
     std::vector<double> tmp(in->partialsElems);
     const double* src = in->partials[bufferIndex];
     double* dTmp = nullptr;
@@ -1454,6 +1634,17 @@ int launchFused(Instance* in, int E, int wIdx, int fIdx, int cum, double* outSum
         pendingOf[in->pendingMats[q].prob] = q;
     }
     A.nOps = (int)in->pendingOps.size();
+    {
+        // k_incremental reads stored partials only: every child not written by an EARLIER op of the list
+        std::vector<int> outside;
+        for (int k = 0; k < A.nOps; ++k)
+            for (int c : {in->pendingOps[k].c1, in->pendingOps[k].c2}) {
+                bool written = false;
+                for (int w = 0; w < k; ++w) written = written || in->pendingOps[w].dest == c;
+                if (!written) outside.push_back(c);
+            }
+        CUDA_OK(storeCherries(in, outside.data(), (int)outside.size()));
+    }
     int prevDest = -1;
     for (int k = 0; k < A.nOps; ++k) {
         const HostOp& o = in->pendingOps[k];
@@ -1482,6 +1673,7 @@ int launchFused(Instance* in, int E, int wIdx, int fIdx, int cum, double* outSum
     A.seq = ++in->incSeq;
     CUDA_OK(launchIncremental(in, A));
     noteScaleWrites(in, in->pendingOps);
+    noteCherryWrites(in, in->pendingOps, {});
     in->pendingMats.clear();
     in->pendingOps.clear();
     in->fusedLaunches++;
@@ -1870,6 +2062,7 @@ static int rootLaunch(Instance* in, int buffer, int wIdx, int fIdx, int cum, int
         !validRange(fIdx, in->nSets))
         return BEAGLE_ERROR_OUT_OF_RANGE;
     if (cum != BEAGLE_OP_NONE && !validRange(cum, in->nScale)) return BEAGLE_ERROR_OUT_OF_RANGE;
+    CUDA_OK(storeCherries(in, &buffer, 1));
     TimedScope ts(in, T_ROOT);
     const Exchange* ex = nullptr;
     if (joint && in->exchangeOn) {          // member of a reduce group: the kernel adds the other shards' sums (Exchange)
@@ -1989,6 +2182,7 @@ int beagleCalculateEdgeDerivatives(int instance, const int* postBufferIndices, c
         edges[e].D = in->dMat + (size_t)dm * in->matStride;
         edges[e].len = 0.0;
     }
+    CUDA_OK(storeCherries(in, postBufferIndices, count));
     // workspace: [edge records][sum, sumSquared per edge][per-pattern values (optional)][tile partials (tensor form)]
     const size_t perEdge = outDerivatives != nullptr ? (size_t)in->P : 0;
     const size_t edgeDoubles = ((size_t)count * sizeof(EdgeRef) + 7) / 8;
@@ -2044,6 +2238,7 @@ int beagleCalculateCrossProductDerivative(int instance, const int* postBufferInd
         edges[e].D = nullptr;
         edges[e].len = edgeLengths[e];
     }
+    CUDA_OK(storeCherries(in, postBufferIndices, count));
     EdgeRef* dEdges = reinterpret_cast<EdgeRef*>(in->dScratch);
     double* work = in->dScratch + edgeDoubles;
     CUDA_OK(cudaMemcpyAsync(dEdges, edges.data(), sizeof(EdgeRef) * count, cudaMemcpyHostToDevice, in->stream));

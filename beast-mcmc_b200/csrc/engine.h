@@ -34,10 +34,13 @@ struct alignas(16) DevOp {
 
 // Compact operation record of the 4-state walk: 64 bytes = four warp-uniform 128-bit loads, all
 // addressing by index so that no pointer has to be chased on the per-op critical path.
-//   dest/c1/c2 : partials slot (>= 0) in the contiguous slab, or -(tipIndex+1) for a compact tip
+//   dest/c1/c2 : partials slot (>= 0) in the contiguous slab, or -(tipIndex+1) for a compact tip; a virtual cherry
+//                child (pad_ bit 2 / 3) is its buffer index, i.e. its row of the recipe table, and its two tips are entry
+//                k of a parallel int4 array (child 1: x, y; child 2: z, w) that only k_walk4pv reads
 //   m1/m2      : transition-matrix buffer index;  sw/sr/cum : scale buffer index or -1
 //   slots      : byte0 srcSlot1, byte1 srcSlot2, byte2 dstSlot of the shared-memory operand stack (0xFF = none)
-//   pad_       : bit 0 = pre-order op, bit 1 = child 1 is the previous op's result (taken from registers)
+//   pad_       : bit 0 = pre-order op, bit 1 = child 1 is the previous op's result (taken from registers),
+//                bit 2 / 3 = child 1 / 2 is a virtual cherry (read by k_walk4pv only, walk4e.cu)
 //   pfA/pfB    : operands of the NEXT op of the walk that are already final in memory, prefetched into L1 while this
 //                op computes: 0 = none, ((slot + 1) << 1) = partials slot, (tip << 1) | 1 = compact tip states
 //   pfM1/pfM2  : the next op's matrix buffers (-1 = none)
@@ -49,6 +52,9 @@ struct alignas(16) Op4 {
     int pad_;
     int pfA, pfB, pfM1, pfM2;
 };
+
+// a virtual cherry: a partials buffer whose value is colA[state of tip1] ⊙ colB[state of tip2] (api.cu, walk4e.cu)
+struct CherryRef { int buf, tip1, tip2; };
 
 // one edge of a calculateEdgeDerivatives call
 struct EdgeRef { const double* post; const int* states; const double* pre; const double* D; double len; };
@@ -63,8 +69,13 @@ struct CachedPlan {
     int n = -1;
     bool byPartition = false, fourPath = false, preOrder = false;
     unsigned long epoch = 0;
+    // [op records | subtree table | snapshot items of the virtual cherries | tips of the virtual children per op]
     void* dBlock = nullptr;
-    size_t capacity = 0, subsOffset = 0;
+    size_t capacity = 0, subsOffset = 0, snapOffset = 0, tipsOffset = 0;
+    // virtual cherries: the ones the list produces (not run; their recipes are snapshot first), and the children read from
+    // outside the list -- as a virtual cherry (tip1 >= 0, must still be that cherry on a hit) or as stored partials
+    std::vector<CherryRef> cherries, external;
+    bool readsVirtual = false;                // some op record names a virtual child: needs the eigen form
     std::vector<int> phaseStart, phaseDepth;
     int maxWindow = 0;
     long lastUse = 0;
@@ -157,6 +168,12 @@ struct Instance {
     int eigenWalk = 1;                        // B200_EIGEN_WALK: 0 = always the matrix-form kernel
     int tipMode = 2;                          // B200_TIP_MODE: compact tips by contraction (0), P column from global (1), shared-memory column table (2)
     int thinTipMode = 3;                     // the same choice for thin (R = 1) phases (B200_THIN_TIP_MODE)
+    // virtual cherries (B200_VIRTUAL_CHERRIES, 4-state CP <= 8): per buffer the tips of the cherry it holds (-1 = real
+    // partials) and whether its partials have been written too; recipe rows [buffer][2][16 * CP]
+    int virtualCherries = 1;
+    std::vector<int> cherryTip1, cherryTip2;
+    std::vector<char> cherryStored;
+    double* dRecipe = nullptr;
     double* dRates = nullptr;                 // [nSets][C]
     std::vector<double> hRates, hWeights, hFreqs;   // host mirrors ([nSets][C], [nSets][C], [nSets][4]; 4-state instances use them)
     double* dWeights = nullptr;               // [nSets][C]
@@ -251,8 +268,16 @@ cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nS
 // walk4e.cu: eigen-form 4-state walk; eigen = [V (16) | V^-1 (16)]; aligned = every op covers [0, Ppad)
 // new V | V^-1 (32 doubles) for the captured eigen-form walk launches of a graph; any failure = the caller re-captures
 cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphNode_t>& kernelNodes, const double* eigen);
+// dVirtTips non-null: the records name virtual cherries whose tips are dVirtTips[op] (an error unless every phase runs on
+// k_walk4p, see walk4pServes)
 cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
-                         const double* eigen);
+                         const double* eigen, const int4* dVirtTips);
+// whether an aligned eigen-form phase of nSubs subtree walks runs on k_walk4p (the kernel that reads virtual cherries)
+bool walk4pServes(const Instance* in, int nSubs, int maxWindow);
+// recipe rows of the virtual cherries a list produces: items (buffer, m1, m2, -)
+cudaError_t launchCherrySnapshot(Instance* in, const int4* dItems, int count);
+// stored partials of virtual cherries: items (slot, buffer, tip 1, tip 2)
+cudaError_t launchCherryStore(Instance* in, const int4* dItems, int count);
 cudaError_t launchWalkGeneric(Instance* in, const DevOp* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder);
 // `partial`: edgeDerivativeWorkspace() doubles when that is non-zero (tensor-pipe form), else nullptr
 size_t edgeDerivativeWorkspace(const Instance* in, int count);

@@ -37,6 +37,8 @@ struct WalkArgs {
     // of the list by value -- kernel parameters live in the constant bank, so V / V^-1 cost neither registers nor LSU
     // traffic (DFMA takes them as uniform-register operands)
     const double* evecs;
+    const double* recipes;     // virtual cherries: [buffer][2][16 * CP], the two P blocks each was computed with
+    const int4* virtTips;      // [op] the tips of its virtual children (child 1: x, y; child 2: z, w)
     double V[16];              // Evec[i][k], rows/columns >= S zero
     double Vi[16];             // Ievc[k][j]
 };

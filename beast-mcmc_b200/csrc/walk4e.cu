@@ -229,7 +229,7 @@ k_walk4e(const WalkArgs A) {
 // Those operands are tiny, warp-uniform and known one op ahead, so each warp runs a two-deep cp.async (LDGSTS) pipeline into
 // its own slice of shared memory: while op k computes, record k+2 and ALL small operands of op k+1 travel global -> shared
 // without touching a register; op k+1 finds them with shared-memory latency.  Per op and warp: three LDGSTS instructions.
-//   ring[4]            op records (64 B), fetched two ops ahead
+//   ring[4]            op records (64 B), fetched two ops ahead (k_walk4pv: with the tips of their virtual children)
 //   stage[k & 1]       mat[child][2][5*CP][2] P block of a tip child: the contiguous [j][CP][i] block in HBM travels as 16-byte
 //                                            pieces, one per lane, and every piece lands where the READS are conflict-free:
 //                                            two half tables (states 0-1 / 2-3) of 16-byte entries indexed c*4 + j, so that
@@ -242,6 +242,13 @@ k_walk4e(const WalkArgs A) {
 //                      st[child][G*R]        state bytes of a tip child for this warp's patterns
 // Child partials that are not forwarded in registers keep the look-ahead L1 prefetch.  Aligned lists only (every op spans
 // [0, Ppad)), thin R = 1 phases included; pattern windows (by-partition lists) use k_walk4e.
+//
+// VIRTUAL CHERRIES (k_walk4pv): a cherry (tip x tip op, no rescaling) is a pure function of two state bytes per pattern and
+// two P blocks, so api.cu does not run it at all: its consumers recompute it where they read it.  A virtual child (Op4 flag
+// bit 2 / 3) names the cherry's buffer, whose recipe row holds the two P blocks ([2][j][CP][i], copied by k_cherry_snapshot
+// when the cherry was produced); its two tips travel in a parallel per-op array (one more lane of the record fetch).  Its staging is that of two tip children (tables
+// mat[ch] / mat[2 + ch], state bytes st[ch] / st[2 + ch]) plus the spectrum of the consumer's branch; its value
+// x = colA ⊙ colB is the very product the cherry op would have stored, so everything downstream is bit-identical.
 __device__ __forceinline__ void cpAsync16(void* smemDst, const void* gmemSrc) {
     const unsigned sAddr = (unsigned)__cvta_generic_to_shared(smemDst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"(sAddr), "l"(gmemSrc) : "memory");
@@ -252,22 +259,24 @@ __device__ __forceinline__ void cpAsyncSmall(void* smemDst, const void* gmemSrc)
     asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" :: "r"(sAddr), "l"(gmemSrc), "n"(BYTES) : "memory");
 }
 
-template <int CP, int R>
+template <int CP, int R, bool VIRT>
 struct WarpStage {
-    static constexpr int G = 32 / CP, NP = G * R;
-    double mat[2][5 * CP * 4];
+    static constexpr int G = 32 / CP, NP = G * R, TABLES = VIRT ? 4 : 2;
+    double mat[TABLES][5 * CP * 4];
     double ev[2][CP * 4];
-    alignas(16) unsigned char st[2][NP < 16 ? 16 : NP];
+    alignas(16) unsigned char st[TABLES][NP < 16 ? 16 : NP];
 };
 
-template <int CP, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
-k_walk4p(const WalkArgs A) {
+template <int CP, int R, bool VIRT>
+__device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     constexpr int G = 32 / CP, NP = G * R;
     constexpr int PIECE = NP < 16 ? NP : 16;                       // state bytes travel in 4-, 8- or 16-byte pieces
     static_assert(NP % PIECE == 0 && (PIECE == 4 || PIECE == 8 || PIECE == 16), "state-byte staging");
-    __shared__ __align__(16) WarpStage<CP, R> stages[4][2];
+    constexpr int TABLES = WarpStage<CP, R, VIRT>::TABLES;
+    constexpr int RECQ = sizeof(Op4) / 16 + (VIRT ? 1 : 0);        // 16-byte pieces of one op record (+ its virtual tips)
+    __shared__ __align__(16) WarpStage<CP, R, VIRT> stages[4][2];
     __shared__ __align__(16) Op4 rings[4][4];
+    __shared__ __align__(16) int4 tipRings[4][VIRT ? 4 : 1];
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));            // volatile: never rematerialised as an S2R inside the loop
     const int wib = threadIdx.x >> 5;
@@ -281,14 +290,26 @@ k_walk4p(const WalkArgs A) {
     const int cc = catValid ? c : 0;
     const size_t off0 = ((size_t)cc * A.Ppad + p0) * 4;
     const int last = range.y - 1, S = A.S;
-    WarpStage<CP, R>* stage = stages[wib];
+    WarpStage<CP, R, VIRT>* stage = stages[wib];
     Op4* ring = rings[wib];
+    int4* tipRing = tipRings[wib];
 
     // the gap column (row 4 of every table), once
-    for (int q = lane; q < 4 * CP * 4; q += 32) {
+    for (int q = lane; q < 2 * TABLES * CP * 4; q += 32) {
         const int tbl = q / (CP * 4), e = q % (CP * 4), gc = e >> 2, i = e & 3;
-        stage[tbl >> 1].mat[tbl & 1][(i >> 1) * 10 * CP + 2 * (4 * CP + gc) + (i & 1)] = (i < S) ? 1.0 : 0.0;
+        stage[tbl / TABLES].mat[tbl % TABLES][(i >> 1) * 10 * CP + 2 * (4 * CP + gc) + (i & 1)] = (i < S) ? 1.0 : 0.0;
     }
+    // P block [j][CP][i] (4 * CP * 4 doubles, contiguous) -> table: piece q = (j, c, half) -> half table, entry c*4 + j
+    auto stageBlock = [&](double* tab, const double* src) {
+#pragma unroll
+        for (int q = lane; q < CP * 8; q += 32)
+            cpAsync16(&tab[(q & 1) * 10 * CP + 2 * (((q >> 1) % CP) * 4 + q / (2 * CP))], src + 2 * q);
+    };
+    // lanes 0 .. RECQ-1: record j into the ring (k_walk4pv: lane 4 brings the tips of its virtual children)
+    auto fetchRecord = [&](int j) {
+        if (VIRT && lane == RECQ - 1) cpAsync16(&tipRing[j & 3], A.virtTips + j);
+        else cpAsync16(reinterpret_cast<char*>(&ring[j & 3]) + 16 * lane, reinterpret_cast<const char*>(A.ops + j) + 16 * lane);
+    };
     // what op j reads beyond partials goes to stage j & 1; reads record j from the ring (it has arrived) ONCE -- the fields
     // the compute part needs travel on in registers (4 shared-memory reads per op instead of 20)
     struct Rec { int dest, c1, c2, sw, sr, flags, pfA, pfB; };
@@ -298,36 +319,48 @@ k_walk4p(const WalkArgs A) {
         const int flags = ring[j & 3].pad_;
         const int2 pf = *reinterpret_cast<const int2*>(&ring[j & 3].pfA);
         const int m2 = rec2.x;
-        WarpStage<CP, R>& sg = stage[j & 1];
+        WarpStage<CP, R, VIRT>& sg = stage[j & 1];
 #pragma unroll
         for (int ch = 0; ch < 2; ++ch) {
             const int child = ch == 0 ? rec.y : rec.z, m = ch == 0 ? rec.w : m2;
+            const bool virt = VIRT && (flags & (4 << ch)) != 0;
             if (child < 0) {
-                const double* src = A.mats + (size_t)m * A.matStride;          // [j][CP][i]: 4 * CP * 4 doubles, contiguous
-#pragma unroll
-                for (int q = lane; q < CP * 8; q += 32)                         // piece q = (j, c, half) -> half table, entry c*4 + j
-                    cpAsync16(&sg.mat[ch][(q & 1) * 10 * CP + 2 * (((q >> 1) % CP) * 4 + q / (2 * CP))], src + 2 * q);
-            } else if (lane < CP * 2) {
-                cpAsync16(&sg.ev[ch][2 * lane], A.evecs + (size_t)m * CP * 4 + 2 * lane);
+                stageBlock(sg.mat[ch], A.mats + (size_t)m * A.matStride);
+            } else {
+                if (virt) {
+                    const double* rcp = A.recipes + (size_t)child * 32 * CP;
+                    stageBlock(sg.mat[ch], rcp);
+                    stageBlock(sg.mat[TABLES - 2 + ch], rcp + 16 * CP);
+                }
+                if (lane < CP * 2) cpAsync16(&sg.ev[ch][2 * lane], A.evecs + (size_t)m * CP * 4 + 2 * lane);
             }
         }
-        // one more instruction: state bytes of the tip children (lanes 4 ..) and, on lanes 0-3, record j + 1
+        // one more instruction: record j + 1 on lanes 0 .. RECQ-1, then the state bytes of the tip children and of the
+        // virtual children's tips (set t = table t)
         constexpr int SL = NP / PIECE;
-        if (lane < 4) {
-            if (j + 1 <= last) cpAsync16(reinterpret_cast<char*>(&ring[(j + 1) & 3]) + 16 * lane,
-                                         reinterpret_cast<const char*>(A.ops + j + 1) + 16 * lane);
-        } else if (lane < 4 + 2 * SL) {
-            const int ch = (lane - 4) / SL, piece = (lane - 4) % SL;
+        auto statePiece = [&](int q) {                             // piece q of all state-byte sets
+            const int t = q / SL, piece = q % SL, ch = t & 1;
             const int child = ch == 0 ? rec.y : rec.z;
-            if (child < 0)
-                cpAsyncSmall<PIECE>(&sg.st[ch][PIECE * piece], A.states + (size_t)(-child - 1) * A.Ppad + pBase + PIECE * piece);
+            int tip = t < 2 && child < 0 ? -child - 1 : -1;
+            if (VIRT && (flags & (4 << ch)) != 0) {
+                const int4 vt = tipRing[j & 3];                      // tips of virtual child 1 (x, y), 2 (z, w)
+                tip = t == 0 ? vt.x : t == 1 ? vt.z : t == 2 ? vt.y : vt.w;
+            }
+            if (tip >= 0) cpAsyncSmall<PIECE>(&sg.st[t][PIECE * piece], A.states + (size_t)tip * A.Ppad + pBase + PIECE * piece);
+        };
+        if (lane < RECQ) {
+            if (j + 1 <= last) fetchRecord(j + 1);
+        } else if (lane < RECQ + TABLES * SL) {
+            statePiece(lane - RECQ);
+        }
+        if constexpr (RECQ + TABLES * SL > 32) {
+            if (lane < RECQ + TABLES * SL - 32) statePiece(lane + 32 - RECQ);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
         return Rec{rec.x, rec.y, rec.z, rec2.y, rec2.z, flags, pf.x, pf.y};
     };
     // prologue: records k0 (and k0+1 through issueOperands), then the operands of k0
-    if (lane < 4) cpAsync16(reinterpret_cast<char*>(&ring[range.x & 3]) + 16 * lane,
-                            reinterpret_cast<const char*>(A.ops + range.x) + 16 * lane);
+    if (lane < RECQ) fetchRecord(range.x);
     asm volatile("cp.async.commit_group;" ::: "memory");
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncwarp();
@@ -345,7 +378,7 @@ k_walk4p(const WalkArgs A) {
     for (int k = range.x; k <= last; ++k) {
         const Rec cur = nxt;
         if (k + 1 <= last) nxt = issueOperands(k + 1);             // travels while op k computes
-        const WarpStage<CP, R>& sg = stage[k & 1];
+        const WarpStage<CP, R, VIRT>& sg = stage[k & 1];
         // look-ahead for the child partials of op k+1 that are not forwarded (never this op's destination)
 #pragma unroll
         for (int w = 0; w < 2; ++w) {
@@ -373,6 +406,7 @@ k_walk4p(const WalkArgs A) {
                 const double2 e01 = ep[0], e23 = ep[1];
                 const double e[4] = {e01.x, e01.y, e23.x, e23.y};
                 const bool fromRegisters = ch == 0 && (cur.flags & 2) != 0;
+                const bool virt = VIRT && (cur.flags & (4 << ch)) != 0;
                 const double* xg = A.partials + (size_t)child * A.stride + off0;
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
@@ -380,6 +414,15 @@ k_walk4p(const WalkArgs A) {
                     if (fromRegisters) {
 #pragma unroll
                         for (int i = 0; i < 4; ++i) x[i] = d[r][i];
+                    } else if (virt) {                                  // the cherry's value, as its op would have stored it
+                        const int symA = sg.st[ch][(lane % G) + r * G], symB = sg.st[TABLES - 2 + ch][(lane % G) + r * G];
+                        const int eA = 2 * (symA < S ? cc * 4 + symA : 4 * CP + cc);
+                        const int eB = 2 * (symB < S ? cc * 4 + symB : 4 * CP + cc);
+                        const double2 aLo = *reinterpret_cast<const double2*>(&sg.mat[ch][eA]);
+                        const double2 aHi = *reinterpret_cast<const double2*>(&sg.mat[ch][10 * CP + eA]);
+                        const double2 bLo = *reinterpret_cast<const double2*>(&sg.mat[TABLES - 2 + ch][eB]);
+                        const double2 bHi = *reinterpret_cast<const double2*>(&sg.mat[TABLES - 2 + ch][10 * CP + eB]);
+                        x[0] = aLo.x * bLo.x; x[1] = aLo.y * bLo.y; x[2] = aHi.x * bHi.x; x[3] = aHi.y * bHi.y;
                     } else {
                         ldg256(xg + (size_t)r * G * 4, x);
                     }
@@ -422,9 +465,61 @@ k_walk4p(const WalkArgs A) {
 }
 
 template <int CP, int R, int MINB>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4p(const WalkArgs A) {
+    walk4pBody<CP, R, false>(A);
+}
+
+// lists that read virtual cherries: twice the tip tables per warp stage
+template <int CP, int R, int MINB>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4pv(const WalkArgs A) {
+    walk4pBody<CP, R, true>(A);
+}
+
+template <int CP, int R, int MINB>
 cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid) {
     k_walk4p<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
+}
+
+// one launch bound only (B200_WALK_MINB does not apply): with 3 blocks ptxas keeps the doubled staging in registers without
+// a spill at every R the virtual kernel serves (R = 8 phases keep their cherries, see walk4pServes)
+template <int CP, int R>
+cudaError_t launchPV(Instance* in, const WalkArgs& A, dim3 grid) {
+    k_walk4pv<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
+    return cudaGetLastError();
+}
+
+// recipe rows [buffer][2][16 * CP] of the virtual cherries a list produces: items (buffer, m1, m2, -)
+__global__ void k_cherry_snapshot(const int4* items, const double* mats, size_t matStride, double* recipes, int blk) {
+    const int4 it = items[blockIdx.x];
+    for (int q = threadIdx.x; q < 2 * blk; q += blockDim.x)
+        recipes[(size_t)it.x * 2 * blk + q] = mats[(size_t)(q < blk ? it.y : it.z) * matStride + q % blk];
+}
+
+// stored partials of virtual cherries, from their recipes: items (slot, buffer, tip 1, tip 2), grid.y strides over them;
+// the same lookups and the same product as k_walk4p's tip tables, so the stored value is the one the cherry op would have
+// written
+__global__ void k_cherry_store(const int4* items, int count, double* partials, size_t stride, const uint8_t* states,
+                               const double* recipes, int S, int C, int CP, int Ppad) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= C * Ppad) return;
+    const int c = q / Ppad, p = q - c * Ppad;
+    for (int k = blockIdx.y; k < count; k += gridDim.y) {
+        const int4 it = items[k];
+        const int sA = states[(size_t)it.z * Ppad + p], sB = states[(size_t)it.w * Ppad + p];
+        const double* ra = recipes + (size_t)it.y * 32 * CP;
+        const double* rb = ra + 16 * CP;
+        double v[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const double a = sA < S ? ra[(sA * CP + c) * 4 + i] : (i < S ? 1.0 : 0.0);
+            const double b = sB < S ? rb[(sB * CP + c) * 4 + i] : (i < S ? 1.0 : 0.0);
+            v[i] = a * b;
+        }
+        stg256(partials + (size_t)it.x * stride + (size_t)q * 4, v);
+    }
 }
 
 template <int CP, int R, bool ALIGNED, int MINB, int TIP>
@@ -436,16 +531,34 @@ cudaError_t launchK(Instance* in, const WalkArgs& A, dim3 grid) {
 // shipped configuration per category count: R in {1, 4} x {aligned, windows}, tips through the shared-memory column table
 // (CP <= 8) or the contraction; CP = 4 (the Gamma-4 workloads the metric is quoted on) additionally carries the tuning space
 // behind B200_WALK_R / B200_WALK_MINB / B200_TIP_MODE
+// patterns per thread of a phase: a thin phase (few walks in flight) is latency-bound, one pattern group per thread gives
+// the most warps per op
+int phaseR(const Instance* in, int nSubs, int maxWindow) {
+    const int G = 32 / in->matCP;
+    const long walks = (long)nSubs * ((maxWindow + G * in->walkR - 1) / (G * in->walkR));
+    if ((in->thinR1 && walks < (long)in->smCount * 8) || in->walkR == 1) return 1;
+    if (in->matCP == 4 && (in->walkR == 8 || in->walkR == 2)) return in->walkR;
+    return 4;
+}
+
+bool stagedWalk(const Instance* in, int R, bool aligned) {
+    const int G = 32 / in->matCP;
+    // predicate-free only when a warp's G*R patterns can never straddle the end of the padded pattern axis
+    return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4 && (R == 1 ? in->thinTipMode : in->tipMode) == 3;
+}
+
 template <int CP, int R>
-cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned) {
+cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
     constexpr int G = 32 / CP;
     constexpr int TIPD = CP <= 8 ? 2 : 0;
     const int warps = (maxWindow + G * R - 1) / (G * R);
     dim3 grid((warps + 3) / 4, nSubs);
-    // predicate-free only when a warp's G*R patterns can never straddle the end of the padded pattern axis
-    if (!aligned || in->Ppad % (G * R) != 0) return launchK<CP, R, false, 4, TIPD>(in, A, grid);
     if constexpr (CP <= 8 && G * R >= 4) {
-        if ((R == 1 ? in->thinTipMode : in->tipMode) == 3) {     // per-warp asynchronous operand staging (k_walk4p)
+        if (stagedWalk(in, R, aligned)) {                          // per-warp asynchronous operand staging (k_walk4p)
+            if (virt) {
+                if constexpr (R == 8) return cudaErrorInvalidValue;
+                else return launchPV<CP, R>(in, A, grid);
+            }
             if constexpr (CP == 4) {
                 // a launch bound of 3 blocks lets ptxas keep its registers without a spill and 4 blocks still fit -- the
                 // fastest setting where it was swept, unless B200_WALK_MINB says otherwise
@@ -457,6 +570,8 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
             return launchP<CP, R, 4>(in, A, grid);
         }
     }
+    if (virt) return cudaErrorInvalidValue;                        // only k_walk4p reads virtual cherries
+    if (!aligned || in->Ppad % (G * R) != 0) return launchK<CP, R, false, 4, TIPD>(in, A, grid);
     if constexpr (CP == 4 && R >= 2) {
         const int minb = in->walkMinBlocks, tip = in->tipMode;
         if (tip == 0) {
@@ -476,22 +591,28 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
 }
 
 template <int CP>
-cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned) {
-    // a thin phase (few walks in flight) is latency-bound: one pattern group per thread gives the most warps per op
-    const long walks = (long)nSubs * ((maxWindow + (32 / CP) * in->walkR - 1) / ((32 / CP) * in->walkR));
-    if ((in->thinR1 && walks < (long)in->smCount * 8) || in->walkR == 1) return launchR<CP, 1>(in, A, nSubs, maxWindow, aligned);
+cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
+    const int R = phaseR(in, nSubs, maxWindow);
+    if (R == 1) return launchR<CP, 1>(in, A, nSubs, maxWindow, aligned, virt);
     if constexpr (CP == 4) {
-        if (in->walkR == 8) return launchR<CP, 8>(in, A, nSubs, maxWindow, aligned);
-        if (in->walkR == 2) return launchR<CP, 2>(in, A, nSubs, maxWindow, aligned);
+        if (R == 8) return launchR<CP, 8>(in, A, nSubs, maxWindow, aligned, virt);
+        if (R == 2) return launchR<CP, 2>(in, A, nSubs, maxWindow, aligned, virt);
     }
-    return launchR<CP, 4>(in, A, nSubs, maxWindow, aligned);
+    return launchR<CP, 4>(in, A, nSubs, maxWindow, aligned, virt);
 }
 
 }  // namespace
 
+bool walk4pServes(const Instance* in, int nSubs, int maxWindow) {
+    if (in->matCP == 0) return false;
+    const int R = phaseR(in, nSubs, maxWindow);
+    return R != 8 && stagedWalk(in, R, true);        // R = 8 (B200_WALK_R=8): the virtual kernel would spill
+}
+
 // eigen: [V (16, row-major Evec[i][k]) | V^-1 (16, Ievc[k][j])], padded to 4 x 4 with zeros
 cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
-                         const double* eigen) {
+                         const double* eigen, const int4* dVirtTips) {
+    const bool virt = dVirtTips != nullptr;
     if (nSubs <= 0) return cudaSuccess;
     WalkArgs A;
     A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
@@ -499,17 +620,34 @@ cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int n
     A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
     A.matStride = in->matStride; A.matMmaOffset = 16 * in->matCP;
     A.evecs = in->dEvec;
+    A.recipes = in->dRecipe;
+    A.virtTips = dVirtTips;
+    if (virt && in->dRecipe == nullptr) return cudaErrorInvalidValue;
     for (int q = 0; q < 16; ++q) { A.V[q] = eigen[q]; A.Vi[q] = eigen[16 + q]; }
     switch (in->matCP) {
 #ifndef B200_W4E_QUICK
-        case 1: return launchCP<1>(in, A, nSubs, maxWindow, aligned);
-        case 2: return launchCP<2>(in, A, nSubs, maxWindow, aligned);
-        case 8: return launchCP<8>(in, A, nSubs, maxWindow, aligned);
-        case 16: return launchCP<16>(in, A, nSubs, maxWindow, aligned);
-        case 32: return launchCP<32>(in, A, nSubs, maxWindow, aligned);
+        case 1: return launchCP<1>(in, A, nSubs, maxWindow, aligned, virt);
+        case 2: return launchCP<2>(in, A, nSubs, maxWindow, aligned, virt);
+        case 8: return launchCP<8>(in, A, nSubs, maxWindow, aligned, virt);
+        case 16: return launchCP<16>(in, A, nSubs, maxWindow, aligned, virt);
+        case 32: return launchCP<32>(in, A, nSubs, maxWindow, aligned, virt);
 #endif
-        default: return launchCP<4>(in, A, nSubs, maxWindow, aligned);
+        default: return launchCP<4>(in, A, nSubs, maxWindow, aligned, virt);
     }
+}
+
+cudaError_t launchCherrySnapshot(Instance* in, const int4* dItems, int count) {
+    if (count <= 0) return cudaSuccess;
+    k_cherry_snapshot<<<count, 128, 0, in->stream>>>(dItems, in->dMat, in->matStride, in->dRecipe, 16 * in->matCP);
+    return cudaGetLastError();
+}
+
+cudaError_t launchCherryStore(Instance* in, const int4* dItems, int count) {
+    if (count <= 0) return cudaSuccess;
+    const dim3 grid((in->C * in->Ppad + 255) / 256, std::min(count, 65535));
+    k_cherry_store<<<grid, 256, 0, in->stream>>>(dItems, count, in->partialsBase, in->partialsElems, in->states8Base,
+                                                 in->dRecipe, in->S, in->C, in->matCP, in->Ppad);
+    return cudaGetLastError();
 }
 
 cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphNode_t>& kernelNodes, const double* eigen) {
@@ -517,6 +655,7 @@ cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphN
         cudaKernelNodeParams kp;
         cudaError_t e = cudaGraphKernelNodeGetParams(node, &kp);
         if (e != cudaSuccess) return e;
+        if (kp.func == reinterpret_cast<void*>(k_cherry_snapshot)) continue;     // carries no eigen system
         if (kp.kernelParams == nullptr || kp.kernelParams[0] == nullptr) return cudaErrorInvalidValue;
         WalkArgs A = *static_cast<const WalkArgs*>(kp.kernelParams[0]);       // every eigen-form walk kernel takes ONE WalkArgs
         for (int q = 0; q < 16; ++q) { A.V[q] = eigen[q]; A.Vi[q] = eigen[16 + q]; }
