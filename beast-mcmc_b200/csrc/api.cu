@@ -28,7 +28,7 @@ std::mutex gMutex;
 std::vector<Instance*> gInstances;
 
 const long kSupportedFlags =
-    BEAGLE_FLAG_PRECISION_DOUBLE | BEAGLE_FLAG_COMPUTATION_SYNCH | BEAGLE_FLAG_EIGEN_REAL |
+    BEAGLE_FLAG_PRECISION_DOUBLE | BEAGLE_FLAG_PRECISION_SINGLE | BEAGLE_FLAG_COMPUTATION_SYNCH | BEAGLE_FLAG_EIGEN_REAL |
     BEAGLE_FLAG_EIGEN_COMPLEX | BEAGLE_FLAG_SCALING_MANUAL | BEAGLE_FLAG_SCALING_DYNAMIC |
     BEAGLE_FLAG_SCALERS_RAW | BEAGLE_FLAG_SCALERS_LOG | BEAGLE_FLAG_VECTOR_NONE | BEAGLE_FLAG_THREADING_NONE |
     BEAGLE_FLAG_PROCESSOR_GPU | BEAGLE_FLAG_FRAMEWORK_CUDA | BEAGLE_FLAG_PARALLELOPS_GRID |
@@ -140,11 +140,11 @@ int uploadSmall(Instance* in, void* dDst, const void* src, size_t bytes) {
 
 // partials live in ONE contiguous slab (index addressing in the walk kernels); a buffer index gets
 // its slot on first use (tips that stay compact never consume one)
-double* ensurePartials(Instance* in, int idx) {
+char* ensurePartials(Instance* in, int idx) {
     if (in->partials[idx] == nullptr) {
         if (in->nextSlot >= in->nSlots) return nullptr;
         in->slotOf[idx] = in->nextSlot++;
-        in->partials[idx] = in->partialsBase + (size_t)in->slotOf[idx] * in->partialsElems;
+        in->partials[idx] = in->partialsBase + (size_t)in->slotOf[idx] * in->partialsElems * in->elemBytes();
     }
     return in->partials[idx];
 }
@@ -193,7 +193,7 @@ void buildResources() {
         snprintf(buf, sizeof buf, "%s", prop.name);
         gResourceStrings.push_back(buf);
         snprintf(buf, sizeof buf, "Global memory (MB): %zu | SMs: %d | compute capability: %d.%d | "
-                 "native walk kernels (sm_90a), double precision",
+                 "native walk kernels (sm_90a), fp64 arithmetic, fp64 or fp32 (4-state) partials",
                  (size_t)(prop.totalGlobalMem >> 20), prop.multiProcessorCount, prop.major, prop.minor);
         gResourceStrings.push_back(buf);
     }
@@ -234,6 +234,7 @@ void buildResources() {
 }
 
 char gImplName[] = "B200-CUDA-Double";
+char gImplNameSingle[] = "B200-CUDA-Single";     // fp32 partials storage, fp64 arithmetic
 char gImplDesc[] = "sm_90a walk kernels: one launch per operation list, shared-memory operand stack";
 
 // ---- op planning ------------------------------------------------------------------------------
@@ -941,9 +942,9 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         } else {
             DevOp& d = dops[pos];
             memset(&d, 0, sizeof d);
-            d.dest = in->partials[o.dest];
-            d.c1 = t1 ? nullptr : in->partials[o.c1];
-            d.c2 = t2 ? nullptr : in->partials[o.c2];
+            d.dest = reinterpret_cast<double*>(in->partials[o.dest]);          // S > 4: always a double instance
+            d.c1 = t1 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c1]);
+            d.c2 = t2 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c2]);
             d.s1 = t1 ? (const void*)in->states32[o.c1] : nullptr;
             d.s2 = t2 ? (const void*)in->states32[o.c2] : nullptr;
             d.m1 = in->dMat + (size_t)o.m1 * in->matStride;
@@ -1110,6 +1111,15 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
         scaleBufferCount < 0 || stateCount > 255)
         return BEAGLE_ERROR_OUT_OF_RANGE;
     if (requirementFlags & ~kSupportedFlags) return BEAGLE_ERROR_NO_RESOURCE;
+    // storage precision: fp32 partials exist for the 4-state walk with C <= 8 (the range of the virtual cherries and the
+    // fused incremental path); a single preference elsewhere is met with a double instance, a requirement is not met
+    const bool singleFits = stateCount <= 4 && categoryCount <= 8;
+    if (requirementFlags & BEAGLE_FLAG_PRECISION_SINGLE) {
+        if (!singleFits || (requirementFlags & BEAGLE_FLAG_PRECISION_DOUBLE)) return BEAGLE_ERROR_NO_RESOURCE;
+    }
+    const bool single = singleFits && ((requirementFlags & BEAGLE_FLAG_PRECISION_SINGLE) ||
+                                       ((preferenceFlags & BEAGLE_FLAG_PRECISION_SINGLE) &&
+                                        !((preferenceFlags | requirementFlags) & BEAGLE_FLAG_PRECISION_DOUBLE)));
     BeagleResourceList* rl = beagleGetResourceList();
     int resource = -1;
     if (resourceList == nullptr || resourceCount <= 0) {
@@ -1156,9 +1166,11 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->Ppad = ((patternCount + 31) / 32) * 32;
     in->nBuffers = partialsBufferCount + compactBufferCount;
     in->nSets = std::max(1, eigenBufferCount);
+    in->single = single;
     in->complexEigen = (requirementFlags | preferenceFlags) & BEAGLE_FLAG_EIGEN_COMPLEX;
     in->logScalers = (requirementFlags | preferenceFlags) & BEAGLE_FLAG_SCALERS_LOG;
-    in->flags = BEAGLE_FLAG_PRECISION_DOUBLE | BEAGLE_FLAG_COMPUTATION_SYNCH | BEAGLE_FLAG_SCALING_MANUAL |
+    in->flags = (single ? BEAGLE_FLAG_PRECISION_SINGLE : BEAGLE_FLAG_PRECISION_DOUBLE) | BEAGLE_FLAG_COMPUTATION_SYNCH |
+                BEAGLE_FLAG_SCALING_MANUAL |
                 BEAGLE_FLAG_VECTOR_NONE | BEAGLE_FLAG_THREADING_NONE | BEAGLE_FLAG_PROCESSOR_GPU |
                 BEAGLE_FLAG_FRAMEWORK_CUDA | BEAGLE_FLAG_PARALLELOPS_GRID |
                 (in->complexEigen ? BEAGLE_FLAG_EIGEN_COMPLEX : BEAGLE_FLAG_EIGEN_REAL) |
@@ -1229,6 +1241,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
         while (in->walkR > 1 && (in->Ppad + G * in->walkR - 1) / (G * in->walkR) < in->smCount) in->walkR >>= 1;
     }
     in->stackDepthMax = std::min(64, std::max(0, envInt("B200_STACK_DEPTH", 12)));
+    if (single) { in->walkVariant = 0; in->stackTail = 0; }     // the experimental walk variants are built for fp64 only
 
     ok = ok && cudaStreamCreateWithFlags(&in->stream, cudaStreamNonBlocking) == cudaSuccess;
     const size_t eigenStride = 2 * (size_t)in->S * in->S + 2 * in->S;
@@ -1284,7 +1297,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
         // every partials buffer the caller may address, else (memory-tight) all but the compact tips
         int want[2] = {in->nPartials, std::max(1, in->nPartials - std::min(in->nCompact, in->tipCount))};
         for (int attempt = 0; attempt < 2 && in->partialsBase == nullptr; ++attempt) {
-            size_t bytes = (size_t)want[attempt] * in->partialsElems * sizeof(double);
+            size_t bytes = (size_t)want[attempt] * in->partialsElems * in->elemBytes();
             if (cudaMalloc(reinterpret_cast<void**>(&in->partialsBase), bytes) == cudaSuccess) in->nSlots = want[attempt];
             else { cudaGetLastError(); in->partialsBase = nullptr; }
         }
@@ -1325,7 +1338,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     if (returnInfo != nullptr) {
         returnInfo->resourceNumber = resource;
         returnInfo->resourceName = rl->list[resource].name;
-        returnInfo->implName = gImplName;
+        returnInfo->implName = single ? gImplNameSingle : gImplName;
         returnInfo->implDescription = gImplDesc;
         returnInfo->flags = in->flags;
     }
@@ -1399,7 +1412,7 @@ int beagleGetTipStates(int instance, int tipIndex, int* outStates) {
 
 static int setPartialsImpl(Instance* in, int bufferIndex, const double* inPartials, bool perCategory) {
     if (!validRange(bufferIndex, in->nBuffers) || inPartials == nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
-    double* dst = ensurePartials(in, bufferIndex);
+    char* dst = ensurePartials(in, bufferIndex);
     if (dst == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
     CUDA_OK(settleCherriesOf(in, bufferIndex));
     if (!in->cherryTip1.empty()) in->cherryTip1[bufferIndex] = -1;
@@ -1414,8 +1427,19 @@ static int setPartialsImpl(Instance* in, int bufferIndex, const double* inPartia
                 for (int i = 0; i < in->S; ++i) row[i] = 1.0;     // padded patterns: harmless, finite
             }
         }
-    CUDA_OK(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * in->partialsElems, cudaMemcpyHostToDevice, in->stream));
-    CUDA_OK(cudaStreamSynchronize(in->stream));
+    if (in->single) {
+        // fp32 storage: the rounding of the walk kernels (walk4.cuh roundCell), a subnormal result becomes a signed zero
+        std::vector<float> narrow(in->partialsElems);
+        for (size_t q = 0; q < narrow.size(); ++q) {
+            const float f = (float)tmp[q];
+            narrow[q] = std::fpclassify(f) == FP_SUBNORMAL ? std::copysign(0.0f, f) : f;
+        }
+        CUDA_OK(cudaMemcpyAsync(dst, narrow.data(), sizeof(float) * narrow.size(), cudaMemcpyHostToDevice, in->stream));
+        CUDA_OK(cudaStreamSynchronize(in->stream));
+    } else {
+        CUDA_OK(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * in->partialsElems, cudaMemcpyHostToDevice, in->stream));
+        CUDA_OK(cudaStreamSynchronize(in->stream));
+    }
     if (in->states32[bufferIndex] != nullptr) in->bufferEpoch++;      // tip -> partials: cached plans are stale
     in->states32[bufferIndex] = nullptr;
     in->states8[bufferIndex] = nullptr;
@@ -1442,16 +1466,33 @@ int beagleGetPartials(int instance, int bufferIndex, int scaleIndex, double* out
     if (scaleIndex != BEAGLE_OP_NONE && !validRange(scaleIndex, in->nScale)) return BEAGLE_ERROR_OUT_OF_RANGE;
     CUDA_OK(storeCherries(in, &bufferIndex, 1));
     std::vector<double> tmp(in->partialsElems);
-    const double* src = in->partials[bufferIndex];
+    const double* src = reinterpret_cast<const double*>(in->partials[bufferIndex]);
     double* dTmp = nullptr;
+    if (in->single) {
+        // fp32 storage: widen here; with a scale index the fp64 unscaling below then runs on the widened copy
+        std::vector<float> narrow(in->partialsElems);
+        CUDA_OK(cudaMemcpyAsync(narrow.data(), in->partials[bufferIndex], sizeof(float) * narrow.size(),
+                                cudaMemcpyDeviceToHost, in->stream));
+        CUDA_OK(cudaStreamSynchronize(in->stream));
+        for (size_t q = 0; q < narrow.size(); ++q) tmp[q] = narrow[q];
+    }
     if (scaleIndex != BEAGLE_OP_NONE) {
         CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&dTmp), sizeof(double) * in->partialsElems));
-        CUDA_OK(cudaMemcpyAsync(dTmp, src, sizeof(double) * in->partialsElems, cudaMemcpyDeviceToDevice, in->stream));
+        if (in->single) {
+            const cudaError_t eUp = cudaMemcpyAsync(dTmp, tmp.data(), sizeof(double) * in->partialsElems,
+                                                    cudaMemcpyHostToDevice, in->stream);
+            if (eUp != cudaSuccess) { cudaFree(dTmp); CUDA_OK(eUp); }
+        } else {
+            CUDA_OK(cudaMemcpyAsync(dTmp, src, sizeof(double) * in->partialsElems, cudaMemcpyDeviceToDevice, in->stream));
+        }
         CUDA_OK(launchRescalePartialsForGet(in, dTmp, in->dScale + (size_t)scaleIndex * in->Ppad));
         src = dTmp;
     }
-    cudaError_t e = cudaMemcpyAsync(tmp.data(), src, sizeof(double) * in->partialsElems, cudaMemcpyDeviceToHost, in->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(in->stream);
+    cudaError_t e = cudaSuccess;
+    if (!in->single || dTmp != nullptr) {          // a single instance without a scale index has tmp already
+        e = cudaMemcpyAsync(tmp.data(), src, sizeof(double) * in->partialsElems, cudaMemcpyDeviceToHost, in->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(in->stream);
+    }
     if (dTmp) cudaFree(dTmp);
     CUDA_OK(e);
     for (int c = 0; c < in->C; ++c)
@@ -2170,7 +2211,7 @@ int beagleCalculateEdgeDerivatives(int instance, const int* postBufferIndices, c
     GET_INSTANCE(in, instance);
     if (count <= 0) return BEAGLE_SUCCESS;
     if (!validRange(categoryWeightsIndices[0], in->nSets)) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<EdgeRef> edges(count);
+    std::vector<EdgeRefT<void>> edges(count);
     for (int e = 0; e < count; ++e) {
         const int po = postBufferIndices[e], pr = preBufferIndices[e], dm = derivativeMatrixIndices[e];
         if (!validRange(po, in->nBuffers) || !validRange(pr, in->nBuffers) || !validRange(dm, in->nMatrices) ||
@@ -2185,13 +2226,13 @@ int beagleCalculateEdgeDerivatives(int instance, const int* postBufferIndices, c
     CUDA_OK(storeCherries(in, postBufferIndices, count));
     // workspace: [edge records][sum, sumSquared per edge][per-pattern values (optional)][tile partials (tensor form)]
     const size_t perEdge = outDerivatives != nullptr ? (size_t)in->P : 0;
-    const size_t edgeDoubles = ((size_t)count * sizeof(EdgeRef) + 7) / 8;
+    const size_t edgeDoubles = ((size_t)count * sizeof(EdgeRefT<void>) + 7) / 8;
     const size_t results = (size_t)count * (2 + perEdge);
     const size_t partials = edgeDerivativeWorkspace(in, count);
     CUDA_OK(ensureScratch(in, edgeDoubles + results + partials));
-    EdgeRef* dEdges = reinterpret_cast<EdgeRef*>(in->dScratch);
+    EdgeRefT<void>* dEdges = reinterpret_cast<EdgeRefT<void>*>(in->dScratch);
     double* dOut = in->dScratch + edgeDoubles;
-    CUDA_OK(cudaMemcpyAsync(dEdges, edges.data(), sizeof(EdgeRef) * count, cudaMemcpyHostToDevice, in->stream));
+    CUDA_OK(cudaMemcpyAsync(dEdges, edges.data(), sizeof(EdgeRefT<void>) * count, cudaMemcpyHostToDevice, in->stream));
     {
         TimedScope ts(in, T_ROOT);
         CUDA_OK(launchEdgeDerivatives(in, dEdges, count, in->dWeights + (size_t)categoryWeightsIndices[0] * in->C,
@@ -2223,10 +2264,10 @@ int beagleCalculateCrossProductDerivative(int instance, const int* postBufferInd
     if (!validRange(categoryRatesIndices[0], in->nSets) || !validRange(categoryWeightsIndices[0], in->nSets))
         return BEAGLE_ERROR_OUT_OF_RANGE;
     const size_t n = (size_t)in->S * in->S;
-    const size_t edgeDoubles = ((size_t)count * sizeof(EdgeRef) + 7) / 8;
+    const size_t edgeDoubles = ((size_t)count * sizeof(EdgeRefT<void>) + 7) / 8;
     const size_t need = edgeDoubles + ((size_t)crossProductBlocks(in, count) + 1) * n;
     CUDA_OK(ensureScratch(in, need));
-    std::vector<EdgeRef> edges(count);
+    std::vector<EdgeRefT<void>> edges(count);
     for (int e = 0; e < count; ++e) {
         const int po = postBufferIndices[e], pr = preBufferIndices[e];
         if (!validRange(po, in->nBuffers) || !validRange(pr, in->nBuffers) || in->partials[pr] == nullptr ||
@@ -2239,9 +2280,9 @@ int beagleCalculateCrossProductDerivative(int instance, const int* postBufferInd
         edges[e].len = edgeLengths[e];
     }
     CUDA_OK(storeCherries(in, postBufferIndices, count));
-    EdgeRef* dEdges = reinterpret_cast<EdgeRef*>(in->dScratch);
+    EdgeRefT<void>* dEdges = reinterpret_cast<EdgeRefT<void>*>(in->dScratch);
     double* work = in->dScratch + edgeDoubles;
-    CUDA_OK(cudaMemcpyAsync(dEdges, edges.data(), sizeof(EdgeRef) * count, cudaMemcpyHostToDevice, in->stream));
+    CUDA_OK(cudaMemcpyAsync(dEdges, edges.data(), sizeof(EdgeRefT<void>) * count, cudaMemcpyHostToDevice, in->stream));
     {
         TimedScope ts(in, T_ROOT);
         CUDA_OK(launchCrossProducts(in, dEdges, count, in->dRates + (size_t)categoryRatesIndices[0] * in->C,

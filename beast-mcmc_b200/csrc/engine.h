@@ -2,7 +2,8 @@
 //
 // One Instance owns every device allocation between beagleCreateInstance and
 // beagleFinalizeInstance.  Device layout (DESIGN.md "Data layout in HBM"):
-//   partials buffer   [C][Ppad][Sp] f64   (Ppad = P rounded up to 32 patterns, Sp = padded states)
+//   partials buffer   [C][Ppad][Sp] f64, or f32 on a PRECISION_SINGLE instance   (Ppad = P rounded up to 32 patterns,
+//                     Sp = padded states)
 //   compact tip       [Ppad] u8 + [Ppad] i32, value S = gap/unknown
 //   transition matrix [C][Sp(child j)][Sp(parent i)] f64  -- stored TRANSPOSED so that a compact-tip
 //                     child reads one contiguous column and lanes indexed by parent state are coalesced
@@ -15,6 +16,7 @@
 
 namespace b200 {
 
+// op record of the generic (S > 4) walk; those instances are always double
 struct alignas(16) DevOp {
     double* dest;
     const double* c1;      // child-1 partials, or nullptr when the child is a compact tip
@@ -57,7 +59,9 @@ struct alignas(16) Op4 {
 struct CherryRef { int buf, tip1, tip2; };
 
 // one edge of a calculateEdgeDerivatives call
-struct EdgeRef { const double* post; const int* states; const double* pre; const double* D; double len; };
+// T = the partials' storage type (float on a PRECISION_SINGLE instance); the host fills EdgeRefT<void>, the same layout
+template <typename T> struct EdgeRefT { const T* post; const int* states; const T* pre; const double* D; double len; };
+using EdgeRef = EdgeRefT<double>;
 
 // a remembered execution plan: the caller's list (key) and its device-resident op records + subtree table
 struct HostOp { int dest, sw, sr, c1, m1, c2, m2, part, cum; int kind = 0; };   // kind 1 = pre-order op
@@ -105,7 +109,7 @@ constexpr int kIncMaxOps = 64, kIncMaxMats = 8;
 struct IncOp { int dest, c1, c2, m1, m2, sw, sr, flags; };      // m < 0: pending branch -(q+1); flags bit 0: c1 = previous result
 struct IncMat { int prob, rateSet; double len; };
 struct IncArgs {
-    double* partials; size_t stride; const uint8_t* states; double* mats; double* evecs; double* scale;
+    void* partials; size_t stride; const uint8_t* states; double* mats; double* evecs; double* scale;
     size_t matStride;
     int S, C, Ppad, P, logScalers, nOps, nMats, pad_;
     double V[16], Vi[16], eval[4];
@@ -143,11 +147,15 @@ struct Instance {
     int smCount = 132;                        // H100 SXM; replaced by the device's count at instance creation
     size_t maxSmemOptin = 0;
 
-    size_t partialsElems = 0;                 // C*Ppad*Sp = stride of one partials slot
-    double* partialsBase = nullptr;           // ONE contiguous slab of nSlots partials buffers
+    // PRECISION_SINGLE (S <= 4, C <= 8): partials are stored as fp32 and every value is rounded to fp32 before it is read;
+    // arithmetic, matrices, scale buffers and everything at the API stay fp64 (DESIGN.md section 4.1)
+    bool single = false;
+    size_t partialsElems = 0;                 // C*Ppad*Sp = stride of one partials slot, in elements
+    size_t elemBytes() const { return single ? sizeof(float) : sizeof(double); }
+    char* partialsBase = nullptr;             // ONE contiguous slab of nSlots partials buffers
     int nSlots = 0, nextSlot = 0;
     std::vector<int> slotOf;                  // buffer index -> slot (assigned on first use), -1 = none
-    std::vector<double*> partials;            // = partialsBase + slot*stride, nullptr while unassigned
+    std::vector<char*> partials;              // = partialsBase + slot*stride*elemBytes(), nullptr while unassigned
     uint8_t* states8Base = nullptr;           // [tipCount][Ppad] compact states (4-state path)
     int* states32Base = nullptr;              // [tipCount][Ppad] compact states (generic path)
     std::vector<uint8_t*> states8;            // non-null while buffer idx is a compact tip
@@ -281,16 +289,16 @@ cudaError_t launchCherryStore(Instance* in, const int4* dItems, int count);
 cudaError_t launchWalkGeneric(Instance* in, const DevOp* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder);
 // `partial`: edgeDerivativeWorkspace() doubles when that is non-zero (tensor-pipe form), else nullptr
 size_t edgeDerivativeWorkspace(const Instance* in, int count);
-cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRef* dEdges, int count, const double* weights, double* outPerPattern,
+cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRefT<void>* dEdges, int count, const double* weights, double* outPerPattern,
                                   double* outSum, double* outSumSq, double* partial);
 // patterns.cu: unique site patterns in first-occurrence order (0 or a negative BEAGLE error code)
 int compressSitePatterns(int device, int taxa, int sites, const int* hStates, int* hPatternOfSite, int* hPatterns,
                          double* hWeights, int* hPatternCount);
 int crossProductBlocks(const Instance* in, int count);
-cudaError_t launchCrossProducts(Instance* in, const EdgeRef* dEdges, int count, const double* rates,
+cudaError_t launchCrossProducts(Instance* in, const EdgeRefT<void>* dEdges, int count, const double* rates,
                                 const double* weights, double* scratch);
 // exchange: non-null = add the other members' sums inside the kernel (dOutSlot[0] = joint value, dOutSlot[1] = local)
-cudaError_t launchRoot(Instance* in, const double* root, const double* weights, const double* freqs,
+cudaError_t launchRoot(Instance* in, const void* root, const double* weights, const double* freqs,
                        const double* cumScale, int pBegin, int pEnd, double* dOutSlot, const Exchange* exchange = nullptr);
 cudaError_t launchIncremental(Instance* in, const IncArgs& args);
 cudaError_t launchCombineMatrices(Instance* in, const int* dFirst, const int* dSecond, const int* dResult, int count, bool multiply);

@@ -25,9 +25,8 @@ __device__ __forceinline__ double absBitsI(double v) {
     return __hiloint2double(__double2hiint(v) & 0x7fffffff, __double2loint(v));
 }
 
-template <int CP>
-__global__ void __launch_bounds__(128)
-k_incremental(const IncArgs A) {
+template <typename T, int CP>
+__device__ __forceinline__ void incrementalBody(const IncArgs& A) {
     constexpr int G = 32 / CP;
     __shared__ double sE[kIncMaxMats][CP][4];
     __shared__ __align__(16) double sP[kIncMaxMats][CP][16];      // [c][j][i]: column j of P_c = contribution of a tip in state j
@@ -54,7 +53,8 @@ k_incremental(const IncArgs A) {
                 if (c == 0) prefetchL1(A.states + (size_t)(-child - 1) * A.Ppad + pp);
                 if (m >= 0 && lane < 4) prefetchL1(A.mats + (size_t)m * A.matStride + lane * 4 * CP);
             } else {
-                if (!(ch == 0 && (op.flags & 1)) && catValid) prefetchL1(A.partials + (size_t)child * A.stride + off0);
+                if (!(ch == 0 && (op.flags & 1)) && catValid)
+                    prefetchL1(static_cast<const T*>(A.partials) + (size_t)child * A.stride + off0);
                 if (m >= 0 && lane == 0) prefetchL1(A.evecs + (size_t)m * CP * 4);
             }
         }
@@ -122,7 +122,7 @@ k_incremental(const IncArgs A) {
 #pragma unroll
                     for (int i = 0; i < 4; ++i) x[i] = d[i];
                 } else {
-                    ldg256(A.partials + (size_t)child * A.stride + off0, x);
+                    loadCell(static_cast<const T*>(A.partials) + (size_t)child * A.stride + off0, x);
                 }
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
@@ -150,7 +150,8 @@ k_incremental(const IncArgs A) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) d[i] *= inv;
         }
-        if (catValid && inRange) stg256(A.partials + (size_t)op.dest * A.stride + off0, d);
+        roundCell<T>(d);                       // also what the next op and the root integration below read
+        if (catValid && inRange) storeCell(static_cast<T*>(A.partials) + (size_t)op.dest * A.stride + off0, d);
     }
 
     // ---- 2. root: site[p] = log(sum_c w_c sum_i pi_i root[c,p,i]) + cum[p]; out = sum_p weight[p] site[p]
@@ -196,11 +197,34 @@ k_incremental(const IncArgs A) {
     }
 }
 
+template <int CP>
+__global__ void __launch_bounds__(128)
+k_incremental(const IncArgs A) {
+    incrementalBody<double, CP>(A);
+}
+
+// fp32 partials storage (PRECISION_SINGLE)
+template <int CP>
+__global__ void __launch_bounds__(128)
+k_incrementals(const IncArgs A) {
+    incrementalBody<float, CP>(A);
+}
+
 }  // namespace
 
 cudaError_t launchIncremental(Instance* in, const IncArgs& A) {
     const int G = 32 / in->matCP;
     const int blocks = (in->Ppad + 4 * G - 1) / (4 * G);
+    if (in->single) {
+        switch (in->matCP) {
+            case 1: k_incrementals<1><<<blocks, 128, 0, in->stream>>>(A); break;
+            case 2: k_incrementals<2><<<blocks, 128, 0, in->stream>>>(A); break;
+            case 4: k_incrementals<4><<<blocks, 128, 0, in->stream>>>(A); break;
+            case 8: k_incrementals<8><<<blocks, 128, 0, in->stream>>>(A); break;
+            default: return cudaErrorInvalidValue;
+        }
+        return cudaGetLastError();
+    }
     switch (in->matCP) {
         case 1: k_incremental<1><<<blocks, 128, 0, in->stream>>>(A); break;
         case 2: k_incremental<2><<<blocks, 128, 0, in->stream>>>(A); break;

@@ -280,7 +280,7 @@ __device__ __forceinline__ void applyMat(const Mat4& M, const double (&x)[4], do
 // matrices in registers and re-uses them for R patterns (R = patterns per thread, strided by G so
 // that every load/store instruction still covers 8 consecutive patterns = 256 contiguous bytes).
 // one child's contribution for the R patterns of this thread: y[r][i] (*)= sum_j P[i][j] x_r[j]
-template <int CP, int R, bool STACK, bool FIRST>
+template <typename T, int CP, int R, bool STACK, bool FIRST>
 __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matIdx, int slot, int moff, size_t off0,
                                           int p0, bool catValid, int pBegin, int pEnd, const double2* stackMem,
                                           int nthreads, double (&y)[R][4]) {
@@ -306,7 +306,7 @@ __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matI
     } else {
         Mat4 M;
         loadMat<CP>(m, M);
-        const double* xg = A.partials + (size_t)child * A.stride + off0;
+        const T* xg = static_cast<const T*>(A.partials) + (size_t)child * A.stride + off0;
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const int p = p0 + r * G;
@@ -317,7 +317,7 @@ __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matI
                 double2 hi = stackMem[((slot * R + r) * 2 + 1) * nthreads + threadIdx.x];
                 x[0] = lo.x; x[1] = lo.y; x[2] = hi.x; x[3] = hi.y;
             } else if (active) {
-                ldg256(xg + (size_t)r * G * 4, x);
+                loadCell(xg + (size_t)r * G * 4, x);
             } else { x[0] = x[1] = x[2] = x[3] = 0.0; }
             applyMat(M, x, v);
 #pragma unroll
@@ -326,9 +326,9 @@ __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matI
     }
 }
 
-template <int CP, int R, bool STACK, int MINB, bool PRE>
-__global__ void __launch_bounds__(128, MINB)
-k_walk4(const WalkArgs A) {
+template <typename T, int CP, int R, bool STACK, bool PRE>
+__device__ __forceinline__ void walk4Body(const WalkArgs& A) {
+    static_assert(sizeof(T) == 8 || !STACK, "the operand-stack variant is built for fp64 partials only");
     constexpr int G = 32 / CP;
     extern __shared__ double2 stackMem[];
     const int lane = threadIdx.x & 31;
@@ -368,7 +368,7 @@ k_walk4(const WalkArgs A) {
                     const uint8_t* t = A.states + (size_t)(pf >> 1) * A.Ppad + p0;
                     if ((lane % G) == 0 && c == 0) prefetchL1(t);          // G*R consecutive bytes: one line
                 } else if (catValid) {
-                    const double* xg = A.partials + (size_t)((pf >> 1) - 1) * A.stride + off0;
+                    const T* xg = static_cast<const T*>(A.partials) + (size_t)((pf >> 1) - 1) * A.stride + off0;
 #pragma unroll
                     for (int r = 0; r < R; ++r)
                         if (p0 + r * G < A.Ppad) prefetchL1(xg + (size_t)r * G * 4);
@@ -393,19 +393,19 @@ k_walk4(const WalkArgs A) {
                     for (int i = 0; i < 4; ++i) d[r][i] = v[i];
                 }
             } else {
-                childTerm<CP, R, STACK, true>(A, cur.c1, cur.m1, s1, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
+                childTerm<T, CP, R, STACK, true>(A, cur.c1, cur.m1, s1, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
             }
-            childTerm<CP, R, STACK, false>(A, cur.c2, cur.m2, s2, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
+            childTerm<T, CP, R, STACK, false>(A, cur.c2, cur.m2, s2, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
         } else {
             // pre-order op: q = pre[parent] (*) (M_sib post[sib]) at the parent, then down the node's own branch
             // with the transposed matrix: pre[node][j] = sum_i q[i] M_node[i][j]
             // (depth-first order inside a subtree walk: when this node is the first child of the previous op's node,
             // pre[parent] is still in d -- flag bit 1 -- and is not re-read)
             double v[R][4];
-            childTerm<CP, R, false, true>(A, cur.c2, cur.m2, 0xFF, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, v);
+            childTerm<T, CP, R, false, true>(A, cur.c2, cur.m2, 0xFF, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, v);
             Mat4 M1;
             loadMat<CP>(A.mats + (size_t)cur.m1 * A.matStride + moff, M1);
-            const double* xg = A.partials + (size_t)cur.c1 * A.stride + off0;
+            const T* xg = static_cast<const T*>(A.partials) + (size_t)cur.c1 * A.stride + off0;
             const bool fromRegisters = (cur.pad_ & 2) != 0;
 #pragma unroll
             for (int r = 0; r < R; ++r) {
@@ -414,7 +414,7 @@ k_walk4(const WalkArgs A) {
                 if (fromRegisters) {
 #pragma unroll
                     for (int i = 0; i < 4; ++i) x[i] = d[r][i];
-                } else if (catValid && p >= cur.pBegin && p < cur.pEnd) ldg256(xg + (size_t)r * G * 4, x);
+                } else if (catValid && p >= cur.pBegin && p < cur.pEnd) loadCell(xg + (size_t)r * G * 4, x);
                 double q[4];
 #pragma unroll
                 for (int i = 0; i < 4; ++i) q[i] = x[i] * v[r][i];
@@ -423,7 +423,7 @@ k_walk4(const WalkArgs A) {
             }
         }
         if (R != 1) nxt = loadOp(A.ops + min(k + 1, last));
-        double* dg = A.partials + (size_t)cur.dest * A.stride + off0;
+        T* dg = static_cast<T*>(A.partials) + (size_t)cur.dest * A.stride + off0;
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const int p = p0 + r * G;
@@ -450,7 +450,8 @@ k_walk4(const WalkArgs A) {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) d[r][i] *= inv;
             }
-            if (active) stg256(dg + (size_t)r * G * 4, d[r]);
+            roundCell<T>(d[r]);
+            if (active) storeCell(dg + (size_t)r * G * 4, d[r]);
             if (STACK && sd != 0xFF) {
                 stackMem[((sd * R + r) * 2 + 0) * nthreads + threadIdx.x] = make_double2(d[r][0], d[r][1]);
                 stackMem[((sd * R + r) * 2 + 1) * nthreads + threadIdx.x] = make_double2(d[r][2], d[r][3]);
@@ -460,8 +461,26 @@ k_walk4(const WalkArgs A) {
     }
 }
 
+template <int CP, int R, bool STACK, int MINB, bool PRE>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4(const WalkArgs A) {
+    walk4Body<double, CP, R, STACK, PRE>(A);
+}
+
+// fp32 partials storage (PRECISION_SINGLE); no operand-stack variant
+template <int CP, int R, int MINB, bool PRE>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4s(const WalkArgs A) {
+    walk4Body<float, CP, R, false, PRE>(A);
+}
+
 template <int CP, int R, bool STACK, int MINB, bool PRE = false>
 static cudaError_t launchWalk4K(Instance* in, const WalkArgs& A, dim3 grid, size_t smem) {
+    if (in->single) {                  // the stack variant never runs on a single instance (walkVariant = stackTail = 0)
+        if constexpr (!STACK && CP <= 8) k_walk4s<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
+        else return cudaErrorInvalidValue;
+        return cudaGetLastError();
+    }
     if (smem > 0 && smem > in->walkSmemConfigured) {
         cudaError_t e = cudaFuncSetAttribute(k_walk4<CP, R, STACK, MINB, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -531,7 +550,7 @@ k_walk4t(const WalkArgs A) {
             const int cb = child == 0 ? cur.c1 : cur.c2;
             const size_t moff = (size_t)(child == 0 ? cur.m1 : cur.m2) * mstride;
             if (cb >= 0) {
-                const double* x = A.partials + (size_t)cb * A.stride + cellOff + t;
+                const double* x = static_cast<const double*>(A.partials) + (size_t)cb * A.stride + cellOff + t;
                 double b[C];
 #pragma unroll
                 for (int c = 0; c < C; ++c) b[c] = __ldg(matB + moff + c * 32);
@@ -591,7 +610,7 @@ k_walk4t(const WalkArgs A) {
         }
         // ---- store: lanes t < 2 own states 2t, 2t+1 (16 B) of pattern g ---------------------------
         {
-            double* dst = A.partials + (size_t)cur.dest * A.stride + cellOff + 2 * t;
+            double* dst = static_cast<double*>(A.partials) + (size_t)cur.dest * A.stride + cellOff + 2 * t;
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const int p = pBase + 8 * r;
@@ -1228,14 +1247,15 @@ cudaError_t launchWalkGeneric(Instance* in, const DevOp* dOps, const int4* dSubs
 // ---------------------------------------------------------------------------------------------
 // d[e,p] = (sum_c w_c sum_j pre[c,p,j] (D_c post)[c,p,j]) / (sum_c w_c sum_j pre[c,p,j] post[c,p,j])
 // (preorder/AbstractBeagleBranchGradientDelegate.java:97-150 states the same reduction in Java).
-__global__ void __launch_bounds__(256)
-k_edge_derivatives(const EdgeRef* __restrict__ edges, const double* __restrict__ weights,
-                   const double* __restrict__ patternWeights, int S, int Sp, int C, int P, int Ppad, int matCP,
-                   int stageD, double* __restrict__ outPerPattern, double* __restrict__ outSum,
-                   double* __restrict__ outSumSq) {
+// T = the partials' storage type (float on a PRECISION_SINGLE instance with S < 4)
+template <typename T>
+__device__ __forceinline__ void edgeDerivativesBody(const EdgeRefT<T>* __restrict__ edges, const double* __restrict__ weights,
+                                                    const double* __restrict__ patternWeights, int S, int Sp, int C, int P,
+                                                    int Ppad, int matCP, int stageD, double* __restrict__ outPerPattern,
+                                                    double* __restrict__ outSum, double* __restrict__ outSumSq) {
     extern __shared__ double smd[];            // D_c[j][k] row-major for all categories (when it fits)
     __shared__ double red1[256], red2[256];
-    const EdgeRef e = edges[blockIdx.x];
+    const EdgeRefT<T> e = edges[blockIdx.x];
     const int tid = threadIdx.x;
     auto dIndex = [&](int c, int j, int k) -> size_t {       // location of D[c][j][k] in the engine's matrix layouts
         return matCP ? ((size_t)k * matCP + c) * 4 + j : ((size_t)c * Sp + k) * Sp + j;
@@ -1252,8 +1272,8 @@ k_edge_derivatives(const EdgeRef* __restrict__ edges, const double* __restrict__
         double num = 0.0, den = 0.0;
         const int s = e.states ? e.states[p] : -1;
         for (int c = 0; c < C; ++c) {
-            const double* pre = e.pre + ((size_t)c * Ppad + p) * Sp;
-            const double* post = e.post ? e.post + ((size_t)c * Ppad + p) * Sp : nullptr;
+            const T* pre = e.pre + ((size_t)c * Ppad + p) * Sp;
+            const T* post = e.post ? e.post + ((size_t)c * Ppad + p) * Sp : nullptr;
             double nc = 0.0, dc = 0.0;
             for (int j = 0; j < S; ++j) {
                 double dp = 0.0, pj;
@@ -1288,15 +1308,34 @@ k_edge_derivatives(const EdgeRef* __restrict__ edges, const double* __restrict__
     if (tid == 0) { outSum[blockIdx.x] = red1[0]; outSumSq[blockIdx.x] = red2[0]; }
 }
 
+__global__ void __launch_bounds__(256)
+k_edge_derivatives(const EdgeRef* __restrict__ edges, const double* __restrict__ weights,
+                   const double* __restrict__ patternWeights, int S, int Sp, int C, int P, int Ppad, int matCP,
+                   int stageD, double* __restrict__ outPerPattern, double* __restrict__ outSum,
+                   double* __restrict__ outSumSq) {
+    edgeDerivativesBody<double>(edges, weights, patternWeights, S, Sp, C, P, Ppad, matCP, stageD, outPerPattern, outSum,
+                                outSumSq);
+}
+
+__global__ void __launch_bounds__(256)
+k_edge_derivatives_f32(const EdgeRefT<float>* __restrict__ edges, const double* __restrict__ weights,
+                       const double* __restrict__ patternWeights, int S, int Sp, int C, int P, int Ppad, int matCP,
+                       int stageD, double* __restrict__ outPerPattern, double* __restrict__ outSum,
+                       double* __restrict__ outSumSq) {
+    edgeDerivativesBody<float>(edges, weights, patternWeights, S, Sp, C, P, Ppad, matCP, stageD, outPerPattern, outSum,
+                               outSumSq);
+}
+
 // 4-state form: grid (256-pattern chunks, edges), a thread owns one (edge, pattern); the C differential matrices of the
 // edge sit in shared memory, the 2 C cell loads of a thread are issued four categories at a time.
-__global__ void __launch_bounds__(256)
-k_edge_derivatives4(const EdgeRef* __restrict__ edges, const double* __restrict__ weights,
-                    const double* __restrict__ patternWeights, int C, int P, int Ppad, int matCP,
-                    double* __restrict__ outPerPattern, double* __restrict__ partial) {
+template <typename T>
+__device__ __forceinline__ void edgeDerivatives4Body(const EdgeRefT<T>* __restrict__ edges, const double* __restrict__ weights,
+                                                     const double* __restrict__ patternWeights, int C, int P, int Ppad,
+                                                     int matCP, double* __restrict__ outPerPattern,
+                                                     double* __restrict__ partial) {
     extern __shared__ double sD[];                  // [C][j][k]
     __shared__ double red[8][2];
-    const EdgeRef e = edges[blockIdx.y];
+    const EdgeRefT<T> e = edges[blockIdx.y];
     const int tid = threadIdx.x, p = blockIdx.x * 256 + tid;
     for (int q = tid; q < C * 16; q += 256) {
         const int c = q >> 4, j = (q >> 2) & 3, k = q & 3;
@@ -1312,8 +1351,8 @@ k_edge_derivatives4(const EdgeRef* __restrict__ edges, const double* __restrict_
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const size_t off = ((size_t)min(c0 + u, C - 1) * Ppad + p) * 4;
-                ldg256_ro(e.pre + off, a[u]);
-                if (e.post) ldg256_ro(e.post + off, b[u]);
+                loadCellRo(e.pre + off, a[u]);
+                if (e.post) loadCellRo(e.post + off, b[u]);
                 else {
 #pragma unroll
                     for (int j = 0; j < 4; ++j) b[u][j] = (s >= 4 || s == j) ? 1.0 : 0.0;
@@ -1352,6 +1391,20 @@ k_edge_derivatives4(const EdgeRef* __restrict__ edges, const double* __restrict_
         for (int w = 0; w < 8; ++w) r += red[w][tid];
         partial[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 2 + tid] = r;
     }
+}
+
+__global__ void __launch_bounds__(256)
+k_edge_derivatives4(const EdgeRef* __restrict__ edges, const double* __restrict__ weights,
+                    const double* __restrict__ patternWeights, int C, int P, int Ppad, int matCP,
+                    double* __restrict__ outPerPattern, double* __restrict__ partial) {
+    edgeDerivatives4Body<double>(edges, weights, patternWeights, C, P, Ppad, matCP, outPerPattern, partial);
+}
+
+__global__ void __launch_bounds__(256)
+k_edge_derivatives4_f32(const EdgeRefT<float>* __restrict__ edges, const double* __restrict__ weights,
+                        const double* __restrict__ patternWeights, int C, int P, int Ppad, int matCP,
+                        double* __restrict__ outPerPattern, double* __restrict__ partial) {
+    edgeDerivatives4Body<float>(edges, weights, patternWeights, C, P, Ppad, matCP, outPerPattern, partial);
 }
 
 // Tensor-pipe form for the state counts of the DMMA walk (Sp = 8 NT): block = 4 warps x 16 patterns of ONE edge.
@@ -1507,12 +1560,19 @@ size_t edgeDerivativeWorkspace(const Instance* in, int count) {
     return mma ? (size_t)count * ((in->P + 63) / 64) * 2 : 0;
 }
 
-cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRef* dEdges, int count, const double* weights,
+cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRefT<void>* dRefs, int count, const double* weights,
                                   double* outPerPattern, double* outSum, double* outSumSq, double* partial) {
+    const EdgeRef* dEdges = reinterpret_cast<const EdgeRef*>(dRefs);
+    const EdgeRefT<float>* dEdgesF = reinterpret_cast<const EdgeRefT<float>*>(dRefs);
     if (partial != nullptr && in->matCP > 0) {
         const int chunks = (in->P + 255) / 256;
-        k_edge_derivatives4<<<dim3(chunks, count), 256, sizeof(double) * 16 * in->C, in->stream>>>(
-            dEdges, weights, in->dPatternWeights, in->C, in->P, in->Ppad, in->matCP, outPerPattern, partial);
+        const dim3 grid(chunks, count);
+        if (in->single)
+            k_edge_derivatives4_f32<<<grid, 256, sizeof(double) * 16 * in->C, in->stream>>>(
+                dEdgesF, weights, in->dPatternWeights, in->C, in->P, in->Ppad, in->matCP, outPerPattern, partial);
+        else
+            k_edge_derivatives4<<<grid, 256, sizeof(double) * 16 * in->C, in->stream>>>(
+                dEdges, weights, in->dPatternWeights, in->C, in->P, in->Ppad, in->matCP, outPerPattern, partial);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         k_edge_sum<<<(count + 127) / 128, 128, 0, in->stream>>>(partial, chunks, count, outSum, outSumSq);
@@ -1532,6 +1592,12 @@ cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRef* dEdges, int count
     const size_t budget = in->maxSmemOptin > 16384 ? in->maxSmemOptin - 8192 : 40000;
     const int stageD = need <= budget ? 1 : 0;
     const size_t smem = stageD ? need : 0;
+    if (in->single) {                  // S < 4 (S = 4 took the form above); C <= 8 keeps smem small
+        k_edge_derivatives_f32<<<count, 256, smem, in->stream>>>(dEdgesF, weights, in->dPatternWeights, in->S, in->Sp, in->C,
+                                                                 in->P, in->Ppad, in->matCP, stageD, outPerPattern, outSum,
+                                                                 outSumSq);
+        return cudaGetLastError();
+    }
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(k_edge_derivatives, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -1550,10 +1616,10 @@ cudaError_t launchEdgeDerivatives(Instance* in, const EdgeRef* dEdges, int count
 // fixed order.
 // ---------------------------------------------------------------------------------------------
 // 4-state: a thread owns a pattern, the 16 accumulators stay in registers across the block's edges.
-__global__ void __launch_bounds__(256)
-k_cross4(const EdgeRef* __restrict__ edges, int count, const double* __restrict__ rates,
-         const double* __restrict__ weights, const double* __restrict__ patternWeights, int C, int P, int Ppad,
-         double* __restrict__ scratch) {
+template <typename T>
+__device__ __forceinline__ void cross4Body(const EdgeRefT<T>* __restrict__ edges, int count, const double* __restrict__ rates,
+                                           const double* __restrict__ weights, const double* __restrict__ patternWeights,
+                                           int C, int P, int Ppad, double* __restrict__ scratch) {
     __shared__ double red[8][16];
     const int tid = threadIdx.x, p = blockIdx.x * 256 + tid;
     double acc[16];
@@ -1562,7 +1628,7 @@ k_cross4(const EdgeRef* __restrict__ edges, int count, const double* __restrict_
     if (p < P) {
         const double wp = patternWeights[p];
         for (int e = blockIdx.y; e < count; e += gridDim.y) {
-            const EdgeRef r = edges[e];
+            const EdgeRefT<T> r = edges[e];
             const int s = r.states ? r.states[p] : -1;
             double num[16], den = 0.0;
 #pragma unroll
@@ -1573,8 +1639,8 @@ k_cross4(const EdgeRef* __restrict__ edges, int count, const double* __restrict_
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     const size_t off = ((size_t)min(c0 + u, C - 1) * Ppad + p) * 4;
-                    ldg256_ro(r.pre + off, a[u]);
-                    if (r.post) ldg256_ro(r.post + off, b[u]);
+                    loadCellRo(r.pre + off, a[u]);
+                    if (r.post) loadCellRo(r.post + off, b[u]);
                     else {
 #pragma unroll
                         for (int j = 0; j < 4; ++j) b[u][j] = (s >= 4 || s == j) ? 1.0 : 0.0;
@@ -1614,12 +1680,28 @@ k_cross4(const EdgeRef* __restrict__ edges, int count, const double* __restrict_
     }
 }
 
+__global__ void __launch_bounds__(256)
+k_cross4(const EdgeRef* __restrict__ edges, int count, const double* __restrict__ rates,
+         const double* __restrict__ weights, const double* __restrict__ patternWeights, int C, int P, int Ppad,
+         double* __restrict__ scratch) {
+    cross4Body<double>(edges, count, rates, weights, patternWeights, C, P, Ppad, scratch);
+}
+
+__global__ void __launch_bounds__(256)
+k_cross4_f32(const EdgeRefT<float>* __restrict__ edges, int count, const double* __restrict__ rates,
+             const double* __restrict__ weights, const double* __restrict__ patternWeights, int C, int P, int Ppad,
+             double* __restrict__ scratch) {
+    cross4Body<float>(edges, count, rates, weights, patternWeights, C, P, Ppad, scratch);
+}
+
 // any state count: a block owns PCH patterns; per (edge, category) the scaled pre tile and the post tile go through
 // shared memory and every thread keeps a 4 x 4 tile of the S x S outer-product sum in registers.
-__global__ void __launch_bounds__(256)
-k_cross_generic(const EdgeRef* __restrict__ edges, int count, const double* __restrict__ rates,
-                const double* __restrict__ weights, const double* __restrict__ patternWeights, int S, int Sp, int C,
-                int P, int Ppad, int PCH, double* __restrict__ scratch) {
+// (also the 4-state form for S < 4, k_cross4 being S = 4 only; T = float on a PRECISION_SINGLE instance)
+template <typename T>
+__device__ __forceinline__ void crossGenericBody(const EdgeRefT<T>* __restrict__ edges, int count,
+                                                 const double* __restrict__ rates, const double* __restrict__ weights,
+                                                 const double* __restrict__ patternWeights, int S, int Sp, int C, int P,
+                                                 int Ppad, int PCH, double* __restrict__ scratch) {
     extern __shared__ double smx[];
     const int S4 = (S + 3) & ~3, nt = S4 / 4, ntiles = nt * nt;
     double* fp = smx;                       // [PCH]  w_p t_e / den_p
@@ -1637,7 +1719,7 @@ k_cross_generic(const EdgeRef* __restrict__ edges, int count, const double* __re
 #pragma unroll
             for (int y = 0; y < 4; ++y) acc[x][y] = 0.0;
         for (int e = blockIdx.y; e < count; e += gridDim.y) {
-            const EdgeRef r = edges[e];
+            const EdgeRefT<T> r = edges[e];
             {   // den_p: 8 lanes per pattern, fixed-order shuffle reduction
                 const int pp = tid >> 3, lane = tid & 7;
                 for (int base = 0; base < np; base += 32) {
@@ -1647,10 +1729,10 @@ k_cross_generic(const EdgeRef* __restrict__ edges, int count, const double* __re
                         const int p = p0 + q;
                         const int s = r.states ? r.states[p] : -1;
                         for (int c = 0; c < C; ++c) {
-                            const double* pre = r.pre + ((size_t)c * Ppad + p) * Sp;
+                            const T* pre = r.pre + ((size_t)c * Ppad + p) * Sp;
                             double dc = 0.0;
                             if (r.post) {
-                                const double* post = r.post + ((size_t)c * Ppad + p) * Sp;
+                                const T* post = r.post + ((size_t)c * Ppad + p) * Sp;
                                 for (int k = lane; k < S; k += 8) dc += pre[k] * post[k];
                             } else if (s < S) {
                                 if (lane == (s & 7)) dc = pre[s];
@@ -1706,6 +1788,20 @@ k_cross_generic(const EdgeRef* __restrict__ edges, int count, const double* __re
                 }
         }
     }
+}
+
+__global__ void __launch_bounds__(256)
+k_cross_generic(const EdgeRef* __restrict__ edges, int count, const double* __restrict__ rates,
+                const double* __restrict__ weights, const double* __restrict__ patternWeights, int S, int Sp, int C,
+                int P, int Ppad, int PCH, double* __restrict__ scratch) {
+    crossGenericBody(edges, count, rates, weights, patternWeights, S, Sp, C, P, Ppad, PCH, scratch);
+}
+
+__global__ void __launch_bounds__(256)
+k_cross_generic_f32(const EdgeRefT<float>* __restrict__ edges, int count, const double* __restrict__ rates,
+                    const double* __restrict__ weights, const double* __restrict__ patternWeights, int S, int Sp, int C,
+                    int P, int Ppad, int PCH, double* __restrict__ scratch) {
+    crossGenericBody(edges, count, rates, weights, patternWeights, S, Sp, C, P, Ppad, PCH, scratch);
 }
 
 // Tensor-pipe form for Sp = 8 NT: out[i][j] += sum_p A[p][i] B[p][j] is a GEMM whose contraction index is the pattern.
@@ -1843,7 +1939,7 @@ k_cross_reduce(const double* __restrict__ scratch, int nBlocks, int n, double* _
 
 // scratch must hold crossProductBlocks() * S * S + S * S doubles; the result lands in the last S * S.
 static void crossGeometry(const Instance* in, int count, int& pch, int& chunks, int& groups, bool& mma) {
-    const bool four = in->Sp == 4;
+    const bool four = in->Sp == 4 && in->S == 4;        // k_cross4 writes S x S = 16 entries per block
     const int nt = in->Sp / 8;
     mma = !four && in->genericMma && in->Sp % 8 == 0 && ((nt >= 1 && nt <= 4) || nt == 8);
     pch = four ? 256 : (mma ? 32 : std::max(1, std::min(32, 2048 / in->S)));
@@ -1860,16 +1956,22 @@ int crossProductBlocks(const Instance* in, int count) {
     return chunks * groups;
 }
 
-cudaError_t launchCrossProducts(Instance* in, const EdgeRef* dEdges, int count, const double* rates,
+cudaError_t launchCrossProducts(Instance* in, const EdgeRefT<void>* dRefs, int count, const double* rates,
                                 const double* weights, double* scratch) {
+    const EdgeRef* dEdges = reinterpret_cast<const EdgeRef*>(dRefs);
+    const EdgeRefT<float>* dEdgesF = reinterpret_cast<const EdgeRefT<float>*>(dRefs);
     int pch, chunks, groups; bool mma;
     crossGeometry(in, count, pch, chunks, groups, mma);
     const int n = in->S * in->S;
     dim3 grid(chunks, groups);
     cudaError_t e = cudaSuccess;
-    if (in->Sp == 4) {
-        k_cross4<<<grid, 256, 0, in->stream>>>(dEdges, count, rates, weights, in->dPatternWeights, in->C, in->P,
-                                               in->Ppad, scratch);
+    if (in->Sp == 4 && in->S == 4) {
+        if (in->single)
+            k_cross4_f32<<<grid, 256, 0, in->stream>>>(dEdgesF, count, rates, weights, in->dPatternWeights, in->C, in->P,
+                                                       in->Ppad, scratch);
+        else
+            k_cross4<<<grid, 256, 0, in->stream>>>(dEdges, count, rates, weights, in->dPatternWeights, in->C, in->P,
+                                                   in->Ppad, scratch);
         e = cudaGetLastError();
     } else if (mma) {
         switch (in->Sp / 8) {
@@ -1886,8 +1988,12 @@ cudaError_t launchCrossProducts(Instance* in, const EdgeRef* dEdges, int count, 
             e = cudaFuncSetAttribute(k_cross_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
         }
-        k_cross_generic<<<grid, 256, smem, in->stream>>>(dEdges, count, rates, weights, in->dPatternWeights, in->S,
-                                                         in->Sp, in->C, in->P, in->Ppad, pch, scratch);
+        if (in->single)
+            k_cross_generic_f32<<<grid, 256, smem, in->stream>>>(dEdgesF, count, rates, weights, in->dPatternWeights, in->S,
+                                                                 in->Sp, in->C, in->P, in->Ppad, pch, scratch);
+        else
+            k_cross_generic<<<grid, 256, smem, in->stream>>>(dEdges, count, rates, weights, in->dPatternWeights, in->S,
+                                                             in->Sp, in->C, in->P, in->Ppad, pch, scratch);
         e = cudaGetLastError();
     }
     if (e != cudaSuccess) return e;
@@ -1939,11 +2045,12 @@ __device__ __forceinline__ void exchangeJoint(const Exchange& ex, double mine, d
     }
 }
 
-__global__ void __launch_bounds__(256)
-k_root(const double* __restrict__ root, const double* __restrict__ weights, const double* __restrict__ freqs,
-       const double* __restrict__ cumScale, const double* __restrict__ patternWeights, int S, int Sp, int C,
-       int Ppad, int pBegin, int pEnd, double* __restrict__ site, double* __restrict__ blockSums,
-       unsigned int* __restrict__ counter, double* __restrict__ out, const Exchange ex) {
+template <typename T>
+__device__ __forceinline__ void rootBody(const T* __restrict__ root, const double* __restrict__ weights,
+                                         const double* __restrict__ freqs, const double* __restrict__ cumScale,
+                                         const double* __restrict__ patternWeights, int S, int Sp, int C, int Ppad, int pBegin,
+                                         int pEnd, double* __restrict__ site, double* __restrict__ blockSums,
+                                         unsigned int* __restrict__ counter, double* __restrict__ out, const Exchange& ex) {
     __shared__ double red[256];
     __shared__ bool last;
     const int p = pBegin + blockIdx.x * blockDim.x + threadIdx.x;
@@ -1993,6 +2100,22 @@ k_root(const double* __restrict__ root, const double* __restrict__ weights, cons
     }
 }
 
+__global__ void __launch_bounds__(256)
+k_root(const double* __restrict__ root, const double* __restrict__ weights, const double* __restrict__ freqs,
+       const double* __restrict__ cumScale, const double* __restrict__ patternWeights, int S, int Sp, int C,
+       int Ppad, int pBegin, int pEnd, double* __restrict__ site, double* __restrict__ blockSums,
+       unsigned int* __restrict__ counter, double* __restrict__ out, const Exchange ex) {
+    rootBody(root, weights, freqs, cumScale, patternWeights, S, Sp, C, Ppad, pBegin, pEnd, site, blockSums, counter, out, ex);
+}
+
+__global__ void __launch_bounds__(256)
+k_root_f32(const float* __restrict__ root, const double* __restrict__ weights, const double* __restrict__ freqs,
+           const double* __restrict__ cumScale, const double* __restrict__ patternWeights, int S, int Sp, int C,
+           int Ppad, int pBegin, int pEnd, double* __restrict__ site, double* __restrict__ blockSums,
+           unsigned int* __restrict__ counter, double* __restrict__ out, const Exchange ex) {
+    rootBody(root, weights, freqs, cumScale, patternWeights, S, Sp, C, Ppad, pBegin, pEnd, site, blockSums, counter, out, ex);
+}
+
 // sum of `n` device values (the per-partition sums of a *ByPartition root call), then the same exchange: one block
 __global__ void __launch_bounds__(64)
 k_exchange_sum(const double* __restrict__ vals, int n, double* __restrict__ out, const Exchange ex) {
@@ -2011,16 +2134,21 @@ cudaError_t launchExchangeSum(Instance* in, const double* dVals, int n, double* 
     return cudaGetLastError();
 }
 
-cudaError_t launchRoot(Instance* in, const double* root, const double* weights, const double* freqs,
+cudaError_t launchRoot(Instance* in, const void* root, const double* weights, const double* freqs,
                        const double* cumScale, int pBegin, int pEnd, double* dOutSlot, const Exchange* exchange) {
     int n = pEnd - pBegin;
     Exchange ex;                       // size 1: no exchange
     if (exchange != nullptr) ex = *exchange;
     if (n <= 0 && ex.size <= 1) return cudaMemsetAsync(dOutSlot, 0, sizeof(double), in->stream);
     int blocks = std::max(1, (n + 255) / 256);       // an empty shard still takes part in the exchange (sum 0)
-    k_root<<<blocks, 256, 0, in->stream>>>(root, weights, freqs, cumScale, in->dPatternWeights, in->S, in->Sp,
-                                           in->C, in->Ppad, pBegin, pEnd, in->dSite, in->dBlockSums,
-                                           in->dCounter, dOutSlot, ex);
+    if (in->single)
+        k_root_f32<<<blocks, 256, 0, in->stream>>>(static_cast<const float*>(root), weights, freqs, cumScale,
+                                                   in->dPatternWeights, in->S, in->Sp, in->C, in->Ppad, pBegin, pEnd,
+                                                   in->dSite, in->dBlockSums, in->dCounter, dOutSlot, ex);
+    else
+        k_root<<<blocks, 256, 0, in->stream>>>(static_cast<const double*>(root), weights, freqs, cumScale,
+                                               in->dPatternWeights, in->S, in->Sp, in->C, in->Ppad, pBegin, pEnd,
+                                               in->dSite, in->dBlockSums, in->dCounter, dOutSlot, ex);
     return cudaGetLastError();
 }
 

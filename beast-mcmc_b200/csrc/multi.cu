@@ -242,6 +242,7 @@ int shardedCreate(Instance* parent, int g, const int* devices, int tipCount, int
             return id;
         }
         sh->child.push_back(id);
+        if (k == 0) parent->flags = d.flags;        // the shards' negotiated flags (precision included)
         if (k == 0 && details != nullptr) *details = d;
     }
     if (g > 1) {

@@ -22,10 +22,42 @@ __device__ __forceinline__ void stg256(double* p, const double (&v)[4]) {
                  :: "l"(p), "d"(v[0]), "d"(v[1]), "d"(v[2]), "d"(v[3]) : "memory");
 }
 
+// ---- the partials cell of one pattern (4 states): the one place on the device that knows the storage format.
+// T = double: 32 bytes as two 128-bit accesses.  T = float (PRECISION_SINGLE instances): 16 bytes as one 128-bit access,
+// widened to double on load.  Arithmetic is fp64 either way.  A float instance rounds every partials value before anyone
+// reads it -- stored, forwarded in registers or recomputed (roundCell) -- so the route a value takes never shows.
+// The rounding is that of cvt.rn.ftz.f32.f64: round to nearest, a subnormal result becomes a zero of the same sign (done
+// here on the integer pipe: ptxas emulates the .ftz of that cvt with an FP64 compare, and the FP64 pipe is the busy one).
+template <typename T>
+__device__ __forceinline__ void roundCell(double (&v)[4]) {
+    if constexpr (sizeof(T) == 4) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            float f;
+            asm("cvt.rn.f32.f64 %0, %1;" : "=f"(f) : "d"(v[i]));
+            const unsigned b = __float_as_uint(f);
+            v[i] = (double)((b & 0x7f800000u) ? f : __uint_as_float(b & 0x80000000u));
+        }
+    }
+}
+__device__ __forceinline__ void loadCell(const double* p, double (&v)[4]) { ldg256(p, v); }
+__device__ __forceinline__ void loadCell(const float* p, double (&v)[4]) {
+    float f[4];
+    asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p) : "memory");
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = f[i];
+}
+// v must have been through roundCell<T>: the narrowing below is then exact
+__device__ __forceinline__ void storeCell(double* p, const double (&v)[4]) { stg256(p, v); }
+__device__ __forceinline__ void storeCell(float* p, const double (&v)[4]) {
+    asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};"
+                 :: "l"(p), "f"((float)v[0]), "f"((float)v[1]), "f"((float)v[2]), "f"((float)v[3]) : "memory");
+}
+
 struct WalkArgs {
     const Op4* ops;
     const int4* subs;          // [subtree] = (first op, one-past-last op, first pattern, one-past-last pattern)
-    double* partials;          // slab base
+    void* partials;            // slab base: double, or float on a PRECISION_SINGLE instance (stride counts elements)
     size_t stride;             // elements per slot
     const uint8_t* states;     // [tip][Ppad]
     const double* mats;        // [matrix][4][CP][4]
@@ -62,6 +94,14 @@ __device__ __forceinline__ void prefetchL1(const void* p) {
 __device__ __forceinline__ void ldg256_ro(const double* p, double (&v)[4]) {
     asm("ld.global.nc.v2.f64 {%0,%1}, [%4];\n\tld.global.nc.v2.f64 {%2,%3}, [%4+16];"
         : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "l"(p));
+}
+// a partials cell an EARLIER launch wrote, on the same non-volatile read-only path
+__device__ __forceinline__ void loadCellRo(const double* p, double (&v)[4]) { ldg256_ro(p, v); }
+__device__ __forceinline__ void loadCellRo(const float* p, double (&v)[4]) {
+    float f[4];
+    asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = f[i];
 }
 
 }  // namespace b200

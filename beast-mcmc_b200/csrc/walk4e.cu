@@ -38,7 +38,7 @@ __device__ __forceinline__ double absBits(double v) {       // |v| on the intege
     return __hiloint2double(__double2hiint(v) & 0x7fffffff, __double2loint(v));
 }
 
-template <int CP, int R, bool ALIGNED, bool FIRST, int TIP>
+template <typename T, int CP, int R, bool ALIGNED, bool FIRST, int TIP>
 __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)[16], int child, int matIdx, bool fromRegisters,
                                            int cc, size_t off0, int p0, bool catValid, int pBegin, int pEnd, double (&d)[R][4],
                                            double* tab) {
@@ -101,7 +101,7 @@ __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)
     double e[4];
     ldg256_ro(A.evecs + ((size_t)matIdx * CP + cc) * 4, e);
     const uint8_t* t = A.states + (size_t)(tip ? -child - 1 : 0) * A.Ppad;
-    const double* xg = A.partials + (size_t)(tip ? 0 : child) * A.stride + off0;
+    const T* xg = static_cast<const T*>(A.partials) + (size_t)(tip ? 0 : child) * A.stride + off0;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const int p = p0 + r * G;
@@ -116,7 +116,7 @@ __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)
 #pragma unroll
             for (int i = 0; i < 4; ++i) x[i] = d[r][i];
         } else if (live) {
-            ldg256(xg + (size_t)r * G * 4, x);
+            loadCell(xg + (size_t)r * G * 4, x);
         } else {
             x[0] = x[1] = x[2] = x[3] = 0.0;
         }
@@ -135,9 +135,8 @@ __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)
     }
 }
 
-template <int CP, int R, bool ALIGNED, int MINB, int TIP>
-__global__ void __launch_bounds__(128, MINB)
-k_walk4e(const WalkArgs A) {
+template <typename T, int CP, int R, bool ALIGNED, int TIP>
+__device__ __forceinline__ void walk4eBody(const WalkArgs& A) {
     constexpr int G = 32 / CP;
     const int lane = threadIdx.x & 31;
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -176,7 +175,7 @@ k_walk4e(const WalkArgs A) {
                 const uint8_t* t = A.states + (size_t)(pf >> 1) * A.Ppad + p0;
                 if ((lane % G) == 0 && c == 0) prefetchL1(t);                  // G*R consecutive bytes: one line
             } else if (catValid) {
-                const double* xg = A.partials + (size_t)((pf >> 1) - 1) * A.stride + off0;
+                const T* xg = static_cast<const T*>(A.partials) + (size_t)((pf >> 1) - 1) * A.stride + off0;
 #pragma unroll
                 for (int r = 0; r < R; ++r)
                     if (ALIGNED || p0 + r * G < A.Ppad) prefetchL1(xg + (size_t)r * G * 4);
@@ -189,10 +188,10 @@ k_walk4e(const WalkArgs A) {
             const int mi = lane < 12 ? cur.pfM1 : cur.pfM2;                     // matrix rows, should a child be a compact tip
             if (mi >= 0) prefetchL1(A.mats + (size_t)mi * A.matStride + (lane & 3) * 4 * CP);
         }
-        childTermE<CP, R, ALIGNED, true, TIP>(A, Vi, cur.c1, cur.m1, (cur.pad_ & 2) != 0, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab1);
-        childTermE<CP, R, ALIGNED, false, TIP>(A, Vi, cur.c2, cur.m2, false, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab2);
+        childTermE<T, CP, R, ALIGNED, true, TIP>(A, Vi, cur.c1, cur.m1, (cur.pad_ & 2) != 0, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab1);
+        childTermE<T, CP, R, ALIGNED, false, TIP>(A, Vi, cur.c2, cur.m2, false, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab2);
         if (R != 1) nxt = loadOp(A.ops + min(k + 1, last));
-        double* dg = A.partials + (size_t)cur.dest * A.stride + off0;
+        T* dg = static_cast<T*>(A.partials) + (size_t)cur.dest * A.stride + off0;
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const int p = p0 + r * G;
@@ -214,10 +213,24 @@ k_walk4e(const WalkArgs A) {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) d[r][i] *= inv;
             }
-            if (active) stg256(dg + (size_t)r * G * 4, d[r]);
+            roundCell<T>(d[r]);
+            if (active) storeCell(dg + (size_t)r * G * 4, d[r]);
         }
         cur = nxt;
     }
+}
+
+template <int CP, int R, bool ALIGNED, int MINB, int TIP>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4e(const WalkArgs A) {
+    walk4eBody<double, CP, R, ALIGNED, TIP>(A);
+}
+
+// fp32 partials storage (PRECISION_SINGLE)
+template <int CP, int R, bool ALIGNED, int MINB, int TIP>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4es(const WalkArgs A) {
+    walk4eBody<float, CP, R, ALIGNED, TIP>(A);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -267,7 +280,7 @@ struct WarpStage {
     alignas(16) unsigned char st[TABLES][NP < 16 ? 16 : NP];
 };
 
-template <int CP, int R, bool VIRT>
+template <typename T, int CP, int R, bool VIRT>
 __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     constexpr int G = 32 / CP, NP = G * R;
     constexpr int PIECE = NP < 16 ? NP : 16;                       // state bytes travel in 4-, 8- or 16-byte pieces
@@ -384,7 +397,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
         for (int w = 0; w < 2; ++w) {
             const int pf = w == 0 ? cur.pfA : cur.pfB;
             if (pf == 0 || (pf & 1) || !catValid) continue;
-            const double* xg = A.partials + (size_t)((pf >> 1) - 1) * A.stride + off0;
+            const T* xg = static_cast<const T*>(A.partials) + (size_t)((pf >> 1) - 1) * A.stride + off0;
 #pragma unroll
             for (int r = 0; r < R; ++r) prefetchL1(xg + (size_t)r * G * 4);
         }
@@ -407,7 +420,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
                 const double e[4] = {e01.x, e01.y, e23.x, e23.y};
                 const bool fromRegisters = ch == 0 && (cur.flags & 2) != 0;
                 const bool virt = VIRT && (cur.flags & (4 << ch)) != 0;
-                const double* xg = A.partials + (size_t)child * A.stride + off0;
+                const T* xg = static_cast<const T*>(A.partials) + (size_t)child * A.stride + off0;
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
                     double x[4], u[4], y[4];
@@ -423,8 +436,9 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
                         const double2 bLo = *reinterpret_cast<const double2*>(&sg.mat[TABLES - 2 + ch][eB]);
                         const double2 bHi = *reinterpret_cast<const double2*>(&sg.mat[TABLES - 2 + ch][10 * CP + eB]);
                         x[0] = aLo.x * bLo.x; x[1] = aLo.y * bLo.y; x[2] = aHi.x * bHi.x; x[3] = aHi.y * bHi.y;
+                        roundCell<T>(x);
                     } else {
-                        ldg256(xg + (size_t)r * G * 4, x);
+                        loadCell(xg + (size_t)r * G * 4, x);
                     }
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
@@ -437,7 +451,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
                 }
             }
         }
-        double* dg = A.partials + (size_t)cur.dest * A.stride + off0;
+        T* dg = static_cast<T*>(A.partials) + (size_t)cur.dest * A.stride + off0;
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const int p = p0 + r * G;
@@ -457,7 +471,8 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) d[r][i] *= inv;
             }
-            if (catValid) stg256(dg + (size_t)r * G * 4, d[r]);
+            roundCell<T>(d[r]);
+            if (catValid) storeCell(dg + (size_t)r * G * 4, d[r]);
         }
         asm volatile("cp.async.wait_group 0;" ::: "memory");      // op k+1's operands and record k+2 have landed
         __syncwarp();
@@ -467,27 +482,41 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4p(const WalkArgs A) {
-    walk4pBody<CP, R, false>(A);
+    walk4pBody<double, CP, R, false>(A);
+}
+
+template <int CP, int R, int MINB>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4ps(const WalkArgs A) {
+    walk4pBody<float, CP, R, false>(A);
 }
 
 // lists that read virtual cherries: twice the tip tables per warp stage
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4pv(const WalkArgs A) {
-    walk4pBody<CP, R, true>(A);
+    walk4pBody<double, CP, R, true>(A);
 }
 
 template <int CP, int R, int MINB>
+__global__ void __launch_bounds__(128, MINB)
+k_walk4pvs(const WalkArgs A) {
+    walk4pBody<float, CP, R, true>(A);
+}
+
+template <typename T, int CP, int R, int MINB>
 cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid) {
-    k_walk4p<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
+    if constexpr (sizeof(T) == 4) k_walk4ps<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
+    else k_walk4p<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
 // one launch bound only (B200_WALK_MINB does not apply): with 3 blocks ptxas keeps the doubled staging in registers without
 // a spill at every R the virtual kernel serves (R = 8 phases keep their cherries, see walk4pServes)
-template <int CP, int R>
+template <typename T, int CP, int R>
 cudaError_t launchPV(Instance* in, const WalkArgs& A, dim3 grid) {
-    k_walk4pv<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
+    if constexpr (sizeof(T) == 4) k_walk4pvs<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
+    else k_walk4pv<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
@@ -501,8 +530,9 @@ __global__ void k_cherry_snapshot(const int4* items, const double* mats, size_t 
 // stored partials of virtual cherries, from their recipes: items (slot, buffer, tip 1, tip 2), grid.y strides over them;
 // the same lookups and the same product as k_walk4p's tip tables, so the stored value is the one the cherry op would have
 // written
-__global__ void k_cherry_store(const int4* items, int count, double* partials, size_t stride, const uint8_t* states,
-                               const double* recipes, int S, int C, int CP, int Ppad) {
+template <typename T>
+__device__ __forceinline__ void cherryStoreBody(const int4* items, int count, T* partials, size_t stride,
+                                                const uint8_t* states, const double* recipes, int S, int C, int CP, int Ppad) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= C * Ppad) return;
     const int c = q / Ppad, p = q - c * Ppad;
@@ -518,13 +548,25 @@ __global__ void k_cherry_store(const int4* items, int count, double* partials, s
             const double b = sB < S ? rb[(sB * CP + c) * 4 + i] : (i < S ? 1.0 : 0.0);
             v[i] = a * b;
         }
-        stg256(partials + (size_t)it.x * stride + (size_t)q * 4, v);
+        roundCell<T>(v);
+        storeCell(partials + (size_t)it.x * stride + (size_t)q * 4, v);
     }
 }
 
-template <int CP, int R, bool ALIGNED, int MINB, int TIP>
+__global__ void k_cherry_store(const int4* items, int count, double* partials, size_t stride, const uint8_t* states,
+                               const double* recipes, int S, int C, int CP, int Ppad) {
+    cherryStoreBody(items, count, partials, stride, states, recipes, S, C, CP, Ppad);
+}
+
+__global__ void k_cherry_store_f32(const int4* items, int count, float* partials, size_t stride, const uint8_t* states,
+                                const double* recipes, int S, int C, int CP, int Ppad) {
+    cherryStoreBody(items, count, partials, stride, states, recipes, S, C, CP, Ppad);
+}
+
+template <typename T, int CP, int R, bool ALIGNED, int MINB, int TIP>
 cudaError_t launchK(Instance* in, const WalkArgs& A, dim3 grid) {
-    k_walk4e<CP, R, ALIGNED, MINB, TIP><<<grid, 128, 0, in->stream>>>(A);
+    if constexpr (sizeof(T) == 4) k_walk4es<CP, R, ALIGNED, MINB, TIP><<<grid, 128, 0, in->stream>>>(A);
+    else k_walk4e<CP, R, ALIGNED, MINB, TIP><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
@@ -547,7 +589,7 @@ bool stagedWalk(const Instance* in, int R, bool aligned) {
     return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4 && (R == 1 ? in->thinTipMode : in->tipMode) == 3;
 }
 
-template <int CP, int R>
+template <typename T, int CP, int R>
 cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
     constexpr int G = 32 / CP;
     constexpr int TIPD = CP <= 8 ? 2 : 0;
@@ -557,48 +599,48 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
         if (stagedWalk(in, R, aligned)) {                          // per-warp asynchronous operand staging (k_walk4p)
             if (virt) {
                 if constexpr (R == 8) return cudaErrorInvalidValue;
-                else return launchPV<CP, R>(in, A, grid);
+                else return launchPV<T, CP, R>(in, A, grid);
             }
             if constexpr (CP == 4) {
                 // a launch bound of 3 blocks lets ptxas keep its registers without a spill and 4 blocks still fit -- the
                 // fastest setting where it was swept, unless B200_WALK_MINB says otherwise
                 const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;
-                if (minb >= 6) return launchP<CP, R, 6>(in, A, grid);
-                if (minb == 5) return launchP<CP, R, 5>(in, A, grid);
-                if (minb == 3) return launchP<CP, R, 3>(in, A, grid);
+                if (minb >= 6) return launchP<T, CP, R, 6>(in, A, grid);
+                if (minb == 5) return launchP<T, CP, R, 5>(in, A, grid);
+                if (minb == 3) return launchP<T, CP, R, 3>(in, A, grid);
             }
-            return launchP<CP, R, 4>(in, A, grid);
+            return launchP<T, CP, R, 4>(in, A, grid);
         }
     }
     if (virt) return cudaErrorInvalidValue;                        // only k_walk4p reads virtual cherries
-    if (!aligned || in->Ppad % (G * R) != 0) return launchK<CP, R, false, 4, TIPD>(in, A, grid);
+    if (!aligned || in->Ppad % (G * R) != 0) return launchK<T, CP, R, false, 4, TIPD>(in, A, grid);
     if constexpr (CP == 4 && R >= 2) {
         const int minb = in->walkMinBlocks, tip = in->tipMode;
         if (tip == 0) {
-            if (minb >= 5) return launchK<CP, R, true, 5, 0>(in, A, grid);
-            if (minb == 3) return launchK<CP, R, true, 3, 0>(in, A, grid);
-            return launchK<CP, R, true, 4, 0>(in, A, grid);
+            if (minb >= 5) return launchK<T, CP, R, true, 5, 0>(in, A, grid);
+            if (minb == 3) return launchK<T, CP, R, true, 3, 0>(in, A, grid);
+            return launchK<T, CP, R, true, 4, 0>(in, A, grid);
         }
         if (tip == 1) {
-            if (minb >= 5) return launchK<CP, R, true, 5, 1>(in, A, grid);
-            return launchK<CP, R, true, 4, 1>(in, A, grid);
+            if (minb >= 5) return launchK<T, CP, R, true, 5, 1>(in, A, grid);
+            return launchK<T, CP, R, true, 4, 1>(in, A, grid);
         }
-        if (minb >= 6) return launchK<CP, R, true, 6, 2>(in, A, grid);
-        if (minb == 5) return launchK<CP, R, true, 5, 2>(in, A, grid);
-        if (minb == 3) return launchK<CP, R, true, 3, 2>(in, A, grid);
+        if (minb >= 6) return launchK<T, CP, R, true, 6, 2>(in, A, grid);
+        if (minb == 5) return launchK<T, CP, R, true, 5, 2>(in, A, grid);
+        if (minb == 3) return launchK<T, CP, R, true, 3, 2>(in, A, grid);
     }
-    return launchK<CP, R, true, 4, TIPD>(in, A, grid);
+    return launchK<T, CP, R, true, 4, TIPD>(in, A, grid);
 }
 
-template <int CP>
+template <typename T, int CP>
 cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
     const int R = phaseR(in, nSubs, maxWindow);
-    if (R == 1) return launchR<CP, 1>(in, A, nSubs, maxWindow, aligned, virt);
+    if (R == 1) return launchR<T, CP, 1>(in, A, nSubs, maxWindow, aligned, virt);
     if constexpr (CP == 4) {
-        if (R == 8) return launchR<CP, 8>(in, A, nSubs, maxWindow, aligned, virt);
-        if (R == 2) return launchR<CP, 2>(in, A, nSubs, maxWindow, aligned, virt);
+        if (R == 8) return launchR<T, CP, 8>(in, A, nSubs, maxWindow, aligned, virt);
+        if (R == 2) return launchR<T, CP, 2>(in, A, nSubs, maxWindow, aligned, virt);
     }
-    return launchR<CP, 4>(in, A, nSubs, maxWindow, aligned, virt);
+    return launchR<T, CP, 4>(in, A, nSubs, maxWindow, aligned, virt);
 }
 
 }  // namespace
@@ -624,15 +666,23 @@ cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int n
     A.virtTips = dVirtTips;
     if (virt && in->dRecipe == nullptr) return cudaErrorInvalidValue;
     for (int q = 0; q < 16; ++q) { A.V[q] = eigen[q]; A.Vi[q] = eigen[16 + q]; }
+    if (in->single) {                                // CP <= 8 only: single instances have C <= 8
+        switch (in->matCP) {
+            case 1: return launchCP<float, 1>(in, A, nSubs, maxWindow, aligned, virt);
+            case 2: return launchCP<float, 2>(in, A, nSubs, maxWindow, aligned, virt);
+            case 8: return launchCP<float, 8>(in, A, nSubs, maxWindow, aligned, virt);
+            default: return launchCP<float, 4>(in, A, nSubs, maxWindow, aligned, virt);
+        }
+    }
     switch (in->matCP) {
 #ifndef B200_W4E_QUICK
-        case 1: return launchCP<1>(in, A, nSubs, maxWindow, aligned, virt);
-        case 2: return launchCP<2>(in, A, nSubs, maxWindow, aligned, virt);
-        case 8: return launchCP<8>(in, A, nSubs, maxWindow, aligned, virt);
-        case 16: return launchCP<16>(in, A, nSubs, maxWindow, aligned, virt);
-        case 32: return launchCP<32>(in, A, nSubs, maxWindow, aligned, virt);
+        case 1: return launchCP<double, 1>(in, A, nSubs, maxWindow, aligned, virt);
+        case 2: return launchCP<double, 2>(in, A, nSubs, maxWindow, aligned, virt);
+        case 8: return launchCP<double, 8>(in, A, nSubs, maxWindow, aligned, virt);
+        case 16: return launchCP<double, 16>(in, A, nSubs, maxWindow, aligned, virt);
+        case 32: return launchCP<double, 32>(in, A, nSubs, maxWindow, aligned, virt);
 #endif
-        default: return launchCP<4>(in, A, nSubs, maxWindow, aligned, virt);
+        default: return launchCP<double, 4>(in, A, nSubs, maxWindow, aligned, virt);
     }
 }
 
@@ -645,8 +695,14 @@ cudaError_t launchCherrySnapshot(Instance* in, const int4* dItems, int count) {
 cudaError_t launchCherryStore(Instance* in, const int4* dItems, int count) {
     if (count <= 0) return cudaSuccess;
     const dim3 grid((in->C * in->Ppad + 255) / 256, std::min(count, 65535));
-    k_cherry_store<<<grid, 256, 0, in->stream>>>(dItems, count, in->partialsBase, in->partialsElems, in->states8Base,
-                                                 in->dRecipe, in->S, in->C, in->matCP, in->Ppad);
+    if (in->single)
+        k_cherry_store_f32<<<grid, 256, 0, in->stream>>>(dItems, count, reinterpret_cast<float*>(in->partialsBase),
+                                                      in->partialsElems, in->states8Base, in->dRecipe, in->S, in->C,
+                                                      in->matCP, in->Ppad);
+    else
+        k_cherry_store<<<grid, 256, 0, in->stream>>>(dItems, count, reinterpret_cast<double*>(in->partialsBase),
+                                                     in->partialsElems, in->states8Base, in->dRecipe, in->S, in->C,
+                                                     in->matCP, in->Ppad);
     return cudaGetLastError();
 }
 
