@@ -175,6 +175,7 @@ _SIGNATURES = {
     "b200HostAlloc": ([_L], C.c_void_p),
     "b200HostFree": ([C.c_void_p], None),
     "b200DebugPlan": ([_I if False else _IP, _I, _I, _I, _I, _I, _I, _I, _IP, _IP, _IP, _IP], _I),
+    "b200DebugStackSlots": ([_IP, _I, _I, _I, _I, _I, _I, _IP, _IP, _IP, _IP], _I),
     "b200RootLogLikelihoodDevice": ([_I, _I, _I, _I, _I, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)], _I),
 }
 

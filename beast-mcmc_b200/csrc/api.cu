@@ -431,11 +431,89 @@ void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, int fixedT
     }
 }
 
+// register forwarding: inside one subtree walk a thread re-reads, as a child, exactly the cell it wrote for the previous
+// op -- flag it (bit 1), with that child moved to position 1 (the product commutes exactly); tip: the op's virtual tips
+void forwardFromPrevious(Op4& d, const Op4& pv, bool preOrder, int4* tip) {
+    if (pv.pBegin != d.pBegin || pv.pEnd != d.pEnd) return;
+    const bool v1 = (d.pad_ & 4) != 0, v2 = (d.pad_ & 8) != 0;
+    if (d.c1 >= 0 && !v1 && d.c1 == pv.dest) d.pad_ |= 2;     // pre-order: pre[parent] is the previous result
+    else if (!preOrder && d.c2 >= 0 && !v2 && d.c2 == pv.dest) {
+        std::swap(d.c1, d.c2); std::swap(d.m1, d.m2);
+        if (tip) *tip = make_int4(tip->z, tip->w, tip->x, tip->y);
+        d.pad_ = (d.pad_ & ~12) | (v1 ? 8 : 0) | 2;
+    }
+}
+
+// ---- sibling stack of the staged eigen walk (k_walk4p, walk4e.cu) -----------------------------------------------------
+// Inside one (subtree, pattern tile) walk a result is taken by the next op from registers, or read back later as the
+// sibling of some op, or read by another walk only.  Results of the second kind also go to a per-warp shared-memory slot:
+// the lowest free one when the result is written, freed at its last read that does not come from registers.  With all
+// `depth` slots taken the value travels through memory as before.  Forwarded, tip, virtual and cross-phase children never
+// take a slot.  Every result is still stored to global memory (other walks, later lists, the root and getPartials read it
+// there), so a kernel that ignores the slot bytes computes the same thing.  Needs the final forwarding flags.
+// subDepth[s]: slots the walk of subtree s uses; fromStack / fromMemory: internal children read from a slot / from memory.
+void assignStackSlots(std::vector<Op4>& ops, const std::vector<Sub>& subs, int depth, std::vector<int>& subDepth,
+                      long& fromStack, long& fromMemory) {
+    // the partials slot child ch is read from in memory, or -1 (tip, virtual cherry, forwarded in registers)
+    auto memoryChild = [](const Op4& d, int ch) -> int {
+        const int c = ch == 0 ? d.c1 : d.c2;
+        if (c < 0 || (d.pad_ & (4 << ch)) || (ch == 0 && (d.pad_ & 2))) return -1;
+        return c;
+    };
+    int keys = 1;
+    for (const Op4& d : ops) keys = std::max(keys, 1 + std::max(d.dest, std::max(d.c1, d.c2)));
+    std::vector<int> lastRead(keys, -1), slotOf(keys, -1), freeAt(keys, -1), lastReadOf(ops.size(), -1);
+    subDepth.assign(subs.size(), 0);
+    for (size_t s = 0; s < subs.size(); ++s) {
+        const int b = subs[s].begin, e = subs[s].end;
+        for (int pos = e - 1; pos >= b; --pos) {                  // last memory read of each result before its rewrite
+            const Op4& d = ops[pos];
+            lastReadOf[pos] = lastRead[d.dest];
+            lastRead[d.dest] = -1;
+            for (int ch = 0; ch < 2; ++ch) {
+                const int c = memoryChild(d, ch);
+                if (c >= 0 && lastRead[c] < 0) lastRead[c] = pos;
+            }
+        }
+        unsigned freeMask = (1u << depth) - 1u;
+        for (int pos = b; pos < e; ++pos) {
+            Op4& d = ops[pos];
+            int src[2] = {0xFF, 0xFF};
+            for (int ch = 0; ch < 2; ++ch) {
+                const int c = memoryChild(d, ch);
+                if (c < 0) continue;
+                if (slotOf[c] >= 0) { src[ch] = slotOf[c]; ++fromStack; } else ++fromMemory;
+            }
+            for (int ch = 0; ch < 2; ++ch) {
+                const int c = memoryChild(d, ch);
+                if (c >= 0 && slotOf[c] >= 0 && freeAt[c] == pos) { freeMask |= 1u << slotOf[c]; slotOf[c] = -1; }
+            }
+            if (slotOf[d.dest] >= 0) { freeMask |= 1u << slotOf[d.dest]; slotOf[d.dest] = -1; }     // stale value
+            int dst = 0xFF;
+            if (lastReadOf[pos] > pos && freeMask != 0) {
+                dst = __builtin_ctz(freeMask);
+                freeMask &= ~(1u << dst);
+                slotOf[d.dest] = dst;
+                freeAt[d.dest] = lastReadOf[pos];
+                subDepth[s] = std::max(subDepth[s], dst + 1);
+            }
+            d.slots = (unsigned)src[0] | ((unsigned)src[1] << 8) | ((unsigned)dst << 16);
+        }
+        for (int pos = b; pos < e; ++pos) {                       // leave no marks for the next subtree
+            const Op4& d = ops[pos];
+            lastRead[d.dest] = slotOf[d.dest] = -1;
+            for (int ch = 0; ch < 2; ++ch) if (memoryChild(d, ch) >= 0) lastRead[memoryChild(d, ch)] = -1;
+        }
+    }
+}
+
 // launch the phases of a prepared plan (device-resident op records + subtree table)
 // eigenSlot >= 0: the 4-state list runs in eigen form (walk4e.cu) with that slot's V / V^-1; aligned: no pattern windows;
-// nSnap: virtual cherries the list produces (their recipes are snapshot first); virt: the records name virtual cherries
+// nSnap: virtual cherries the list produces (their recipes are snapshot first); virt: the records name virtual cherries;
+// phaseSlots: sibling-stack depth of each phase (eigen-form walks)
 cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const std::vector<int>& phaseStart,
-                       const std::vector<int>& phaseDepth, bool fourPath, int maxWindow, bool preOrder, int eigenSlot = -1,
+                       const std::vector<int>& phaseDepth, const std::vector<int>& phaseSlots, bool fourPath, int maxWindow,
+                       bool preOrder, int eigenSlot = -1,
                        bool aligned = false, const void* dSnap = nullptr, int nSnap = 0, const void* dVirtTips = nullptr) {
     const bool virt = dVirtTips != nullptr;
     cudaError_t e = cudaSuccess;
@@ -449,7 +527,8 @@ cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const 
         TimedScope ts(in, T_PARTIALS);
         if (fourPath && eigenSlot >= 0 && !preOrder && (ph >= phaseDepth.size() || phaseDepth[ph] == 0)) {
             e = launchWalk4E(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
-                             aligned, in->hEigen.data() + (size_t)eigenSlot * 36, static_cast<const int4*>(dVirtTips));
+                             aligned, in->hEigen.data() + (size_t)eigenSlot * 36, static_cast<const int4*>(dVirtTips),
+                             ph < phaseSlots.size() ? phaseSlots[ph] : 0);
             continue;
         }
         if (virt) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
@@ -623,7 +702,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                 if (cp.graphExec == nullptr && !cp.graphFailed && cp.hits >= 2 && !in->timing &&
                     cudaStreamBeginCapture(in->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
                     const cudaError_t e1 = launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart,
-                                                      cp.phaseDepth, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
+                                                      cp.phaseDepth, cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
                                                       !cp.byPartition, dSnap, nSnap, dTips);
                     cp.graphEigen = eigenSlot;
                     cp.graphEigenGen = eigenGenNow;
@@ -664,7 +743,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                 }
             }
             CUDA_OK(launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart, cp.phaseDepth,
-                               cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap,
+                               cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap,
                                dTips));
             CUDA_OK(accumulateInList(in, cp.cumGroups));
             noteScaleWrites(in, hops);
@@ -926,19 +1005,8 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             d.pfA = d.pfB = 0; d.pfM1 = d.pfM2 = -1;
             if (readsVirtual)
                 virtTips[pos] = make_int4(v1 ? vt1[o.c1] : 0, v1 ? vt2[o.c1] : 0, v2 ? vt1[o.c2] : 0, v2 ? vt2[o.c2] : 0);
-            // register forwarding: inside one subtree walk a thread re-reads, as a child, exactly the cell it wrote for
-            // the previous op -- flag it (bit 1), with that child moved to position 1 (the product commutes exactly)
-            if (in->forward && !(maxDepth > 0 && subStack[subOfPos[pos]]) && pos > plan.subs[subOfPos[pos]].begin) {
-                const Op4& pv = ops4[pos - 1];
-                if (pv.pBegin == d.pBegin && pv.pEnd == d.pEnd) {
-                    if (!t1 && !v1 && d.c1 == pv.dest) d.pad_ |= 2;     // pre-order: pre[parent] is the previous result
-                    else if (!preOrder && !t2 && !v2 && d.c2 == pv.dest) {
-                        std::swap(d.c1, d.c2); std::swap(d.m1, d.m2);
-                        if (readsVirtual) { int4& t = virtTips[pos]; t = make_int4(t.z, t.w, t.x, t.y); }
-                        d.pad_ = (d.pad_ & ~12) | (v1 ? 8 : 0) | 2;
-                    }
-                }
-            }
+            if (in->forward && !(maxDepth > 0 && subStack[subOfPos[pos]]) && pos > plan.subs[subOfPos[pos]].begin)
+                forwardFromPrevious(d, ops4[pos - 1], preOrder, readsVirtual ? &virtTips[pos] : nullptr);
         } else {
             DevOp& d = dops[pos];
             memset(&d, 0, sizeof d);
@@ -968,6 +1036,15 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             }
         }
     }
+    // sibling stack: lists whose phases the staged eigen walk may run (post-order, aligned, no matrix-form stack)
+    std::vector<int> phaseSlots(std::max(nPhases, 1), 0);
+    long fromStack = 0, fromMemory = 0;
+    if (fourPath && eigenSlot >= 0 && !preOrder && !byPartition && maxDepth == 0 && in->stackSlots > 0 && walkStackBuilt(in)) {
+        std::vector<int> subDepth;
+        assignStackSlots(ops4, plan.subs, in->stackSlots, subDepth, fromStack, fromMemory);
+        for (int ph = 0; ph < nPhases; ++ph)
+            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) phaseSlots[ph] = std::max(phaseSlots[ph], subDepth[q]);
+    }
     if (fourPath && in->lookahead && (!preOrder || in->lookaheadPre)) {
         // look-ahead fields: what op k+1 of the same walk will read from memory, except op k's own destination
         // only where the phase is throughput-bound; a thin phase is a pure latency chain and the extra instructions cost
@@ -983,13 +1060,13 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             for (int pos = plan.subs[sIdx].begin; pos + 1 < plan.subs[sIdx].end; ++pos) {
                 Op4& d = ops4[pos];
                 const Op4& nx = ops4[pos + 1];
-                auto enc = [&](int child, bool fromRegisters, bool virt) -> int {
-                    if (fromRegisters || virt) return 0;
+                auto enc = [&](int child, bool fromRegisters, bool virt, bool fromStack) -> int {
+                    if (fromRegisters || virt || fromStack) return 0;
                     if (child < 0) return ((-child - 1) << 1) | 1;
                     return child == d.dest ? 0 : ((child + 1) << 1);
                 };
-                d.pfA = enc(nx.c1, (nx.pad_ & 2) != 0, (nx.pad_ & 4) != 0);
-                d.pfB = enc(nx.c2, false, (nx.pad_ & 8) != 0);
+                d.pfA = enc(nx.c1, (nx.pad_ & 2) != 0, (nx.pad_ & 4) != 0, (nx.slots & 0xFF) != 0xFF);
+                d.pfB = enc(nx.c2, false, (nx.pad_ & 8) != 0, ((nx.slots >> 8) & 0xFF) != 0xFF);
                 if (d.pfA == 0) { d.pfA = d.pfB; d.pfB = 0; }
                 d.pfM1 = nx.m1; d.pfM2 = nx.m2;
             }
@@ -999,7 +1076,8 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         int fwd = 0, internal = 0;
         for (const Op4& d : ops4) { fwd += (d.pad_ & 2) != 0; internal += (d.c1 >= 0) + (d.c2 >= 0); }
         fprintf(stderr, "[b200-beagle] plan: %d ops (%zu virtual cherries), %zu subtrees, %d phases, %d internal children, "
-                "%d forwarded in registers\n", nL, cherries.size(), plan.subs.size(), nPhases, internal, fwd);
+                "%d forwarded in registers, %ld read from the stack, %ld from memory\n", nL, cherries.size(), plan.subs.size(),
+                nPhases, internal, fwd, fromStack, fromMemory);
     }
     // one block: [op records | subtree table | snapshot items], each part 256-byte aligned
     const size_t opBytes = (fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)nL;
@@ -1028,7 +1106,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     void* dSubs = static_cast<char*>(dOps) + subsOffset;
     std::vector<int> depths(plan.phaseStart.size(), 0);
     for (size_t ph = 0; ph + 1 < plan.phaseStart.size(); ++ph) depths[ph] = (maxDepth > 0 && ph < phaseDepth.size()) ? phaseDepth[ph] : 0;
-    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, depths, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
+    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, depths, phaseSlots, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
                                static_cast<char*>(dOps) + snapOffset, (int)snap.size(),
                                readsVirtual ? static_cast<char*>(dOps) + tipsOffset : nullptr);
     if (e == cudaSuccess) e = accumulateInList(in, cumGroups);
@@ -1057,6 +1135,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             slot->subsOffset = subsOffset; slot->snapOffset = snapOffset; slot->tipsOffset = tipsOffset;
             slot->cherries = cherries; slot->external = external; slot->readsVirtual = readsVirtual;
             slot->phaseStart = plan.phaseStart; slot->phaseDepth = depths;
+            slot->phaseSlots = phaseSlots;
             slot->fourPath = fourPath; slot->maxWindow = maxWindow; slot->preOrder = preOrder;
             slot->lastUse = ++in->planClock;
             slot->cumGroups = cumGroups;
@@ -1211,6 +1290,8 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->walkVariant = envInt("B200_WALK_VARIANT", 0);
     in->reorder = envInt("B200_REORDER", 1);
     in->forward = envInt("B200_FORWARD", 1);
+    in->stackSlots = envInt("B200_WALK_STACK_SLOTS", 1) != 0 ? kStackSlots : 0;
+    in->debugLog = getenv("B200_BEAGLE_DEBUG") != nullptr;
     in->lookahead = envInt("B200_LOOKAHEAD", 1);
     in->useGraphs = envInt("B200_GRAPHS", 1);
     in->prePhases = envInt("B200_PRE_PHASES", 1);
@@ -2317,6 +2398,49 @@ int b200DebugPlan(const int* operations, int operationCount, int bufferCount, in
     for (size_t q = 0; q < plan.phaseStart.size(); ++q) outPhaseStart[q] = plan.phaseStart[q];
     outCounts[0] = (int)plan.subs.size();
     outCounts[1] = (int)plan.phaseStart.size() - 1;
+    return BEAGLE_SUCCESS;
+}
+
+// ---- host-logic test hook (no CUDA calls): register forwarding and sibling-stack slots of a post-order list -----------
+int b200DebugStackSlots(const int* operations, int operationCount, int bufferCount, int tipCount, int wantSubs, int minT,
+                        int smallRemainder, int* outRecords, int* outSubs, int* outPhaseStart, int* outCounts) {
+    if (operationCount <= 0 || bufferCount <= 0 || tipCount < 0 || tipCount > bufferCount) return BEAGLE_ERROR_OUT_OF_RANGE;
+    std::vector<HostOp> hops(operationCount);
+    for (int k = 0; k < operationCount; ++k) {
+        const int* o = operations + 7 * k;
+        for (int f : {o[0], o[3], o[5]}) if (f < 0 || f >= bufferCount) return BEAGLE_ERROR_OUT_OF_RANGE;
+        hops[k] = {o[0], o[1], o[2], o[3], o[4], o[5], o[6], 0, -1};
+    }
+    Plan plan;
+    planPhases(hops, bufferCount, true, 0, std::max(1, wantSubs), std::max(1, minT), smallRemainder, plan);
+    std::vector<Op4> ops(operationCount);
+    for (int pos = 0; pos < operationCount; ++pos) {            // buffers below tipCount are compact tips
+        const HostOp& o = hops[plan.order[pos]];
+        Op4& d = ops[pos];
+        memset(&d, 0, sizeof d);
+        d.dest = o.dest;
+        d.c1 = o.c1 < tipCount ? -(o.c1 + 1) : o.c1;
+        d.c2 = o.c2 < tipCount ? -(o.c2 + 1) : o.c2;
+        d.m1 = o.m1; d.m2 = o.m2; d.pEnd = 1;
+        d.slots = 0xFFFFFFu;
+    }
+    for (size_t s = 0; s < plan.subs.size(); ++s)
+        for (int pos = plan.subs[s].begin + 1; pos < plan.subs[s].end; ++pos) forwardFromPrevious(ops[pos], ops[pos - 1], false, nullptr);
+    std::vector<int> subDepth;
+    long fromStack = 0, fromMemory = 0;
+    assignStackSlots(ops, plan.subs, kStackSlots, subDepth, fromStack, fromMemory);
+    for (int pos = 0; pos < operationCount; ++pos) {
+        const Op4& d = ops[pos];
+        int* r = outRecords + 5 * pos;
+        r[0] = d.dest; r[1] = d.c1; r[2] = d.c2; r[3] = d.pad_; r[4] = (int)d.slots;
+    }
+    for (size_t q = 0; q < plan.subs.size(); ++q) { outSubs[2 * q] = plan.subs[q].begin; outSubs[2 * q + 1] = plan.subs[q].end; }
+    for (size_t q = 0; q < plan.phaseStart.size(); ++q) outPhaseStart[q] = plan.phaseStart[q];
+    outCounts[0] = (int)plan.subs.size();
+    outCounts[1] = (int)plan.phaseStart.size() - 1;
+    outCounts[2] = (int)fromStack;
+    outCounts[3] = (int)fromMemory;
+    outCounts[4] = *std::max_element(subDepth.begin(), subDepth.end());
     return BEAGLE_SUCCESS;
 }
 

@@ -80,7 +80,7 @@ struct CachedPlan {
     // outside the list -- as a virtual cherry (tip1 >= 0, must still be that cherry on a hit) or as stored partials
     std::vector<CherryRef> cherries, external;
     bool readsVirtual = false;                // some op record names a virtual child: needs the eigen form
-    std::vector<int> phaseStart, phaseDepth;
+    std::vector<int> phaseStart, phaseDepth, phaseSlots;      // phaseSlots: sibling-stack depth per phase
     int maxWindow = 0;
     long lastUse = 0;
     long hits = 0;
@@ -136,6 +136,11 @@ struct Exchange {
     long long timeoutCycles = 0;             // spin budget (SM clocks) before giving up with NaN
     ExchangeSlot* peers[kMaxGroup] = {};     // member q's slot array as mapped on this device (peers[rank] = own)
 };
+
+// slots per warp of the sibling stack (built into the CP = 4 staged walk at its default launch bound of 3 blocks only,
+// walk4e.cu::stackBuilt): at R = 4 one slot is 4 KB per warp, and three of them keep the 3 blocks per SM the registers allow
+// inside the 228 KB of shared memory; in the cfg-2 and Makona-like plans three slots hold every sibling a walk reads back
+constexpr int kStackSlots = 3;
 
 struct Instance {
     int id = -1, device = 0, resource = 0;
@@ -199,6 +204,10 @@ struct Instance {
     int useGraphs = 1;                        // B200_GRAPHS
     int lookahead = 1;                        // L1 prefetch of the next op's operands (B200_LOOKAHEAD)
     int forward = 1;                          // register forwarding between consecutive ops of a walk (B200_FORWARD)
+    // slots per warp of the staged eigen walk's sibling stack (api.cu::assignStackSlots); B200_WALK_STACK_SLOTS=0 turns
+    // it off, the reference route of the bit-equality tests
+    int stackSlots = kStackSlots;
+    bool debugLog = false;                    // B200_BEAGLE_DEBUG: per-launch diagnostics on stderr
     double* dScratch = nullptr;               // grow-only workspace of the derivative calls
     size_t scratchDoubles = 0;
     int partitionCount = 1;
@@ -277,11 +286,13 @@ cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nS
 // new V | V^-1 (32 doubles) for the captured eigen-form walk launches of a graph; any failure = the caller re-captures
 cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphNode_t>& kernelNodes, const double* eigen);
 // dVirtTips non-null: the records name virtual cherries whose tips are dVirtTips[op] (an error unless every phase runs on
-// k_walk4p, see walk4pServes)
+// k_walk4p, see walk4pServes); stackSlots: slots per warp of the sibling stack the records use (k_walk4p only, 0 = none)
 cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
-                         const double* eigen, const int4* dVirtTips);
+                         const double* eigen, const int4* dVirtTips, int stackSlots);
 // whether an aligned eigen-form phase of nSubs subtree walks runs on k_walk4p (the kernel that reads virtual cherries)
 bool walk4pServes(const Instance* in, int nSubs, int maxWindow);
+// whether the staged-walk kernels this instance launches carry the sibling stack (otherwise they ignore the slot bytes)
+bool walkStackBuilt(const Instance* in);
 // recipe rows of the virtual cherries a list produces: items (buffer, m1, m2, -)
 cudaError_t launchCherrySnapshot(Instance* in, const int4* dItems, int count);
 // stored partials of virtual cherries: items (slot, buffer, tip 1, tip 2)

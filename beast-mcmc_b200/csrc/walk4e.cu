@@ -21,6 +21,9 @@
 //
 // ALIGNED = every op spans whole 32-pattern groups [0, Ppad): no per-pattern predicates at all (padded columns hold
 // harmless finite values and are never read back).  Partition windows take the predicated instance.
+#include <atomic>
+#include <cstdio>
+
 #include "engine.h"
 #include "walk4.cuh"
 
@@ -262,6 +265,12 @@ k_walk4es(const WalkArgs A) {
 // when the cherry was produced); its two tips travel in a parallel per-op array (one more lane of the record fetch).  Its staging is that of two tip children (tables
 // mat[ch] / mat[2 + ch], state bytes st[ch] / st[2 + ch]) plus the spectrum of the consumer's branch; its value
 // x = colA ⊙ colB is the very product the cherry op would have stored, so everything downstream is bit-identical.
+//
+// SIBLING STACK: a result that a later op of the same walk reads, but not from registers (the sibling of some later op),
+// is also kept in a per-warp slot of dynamic shared memory (Op4 slot bytes, assigned by api.cu::assignStackSlots), and
+// that later op reads the slot instead of global memory.  Layout [slot][warp][R][2][32] 16-byte entries: lane fastest,
+// so every STS.128 / LDS.128 is conflict-free.  A thread reads back only cells it wrote itself: program order suffices.
+// The slot holds the rounded cell that was stored, so the value does not depend on the route it takes.
 __device__ __forceinline__ void cpAsync16(void* smemDst, const void* gmemSrc) {
     const unsigned sAddr = (unsigned)__cvta_generic_to_shared(smemDst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"(sAddr), "l"(gmemSrc) : "memory");
@@ -272,6 +281,26 @@ __device__ __forceinline__ void cpAsyncSmall(void* smemDst, const void* gmemSrc)
     asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" :: "r"(sAddr), "l"(gmemSrc), "n"(BYTES) : "memory");
 }
 
+// one cell of the sibling stack: two 16-byte entries 32 entries (one per lane) apart.  volatile, like the global cell
+// accesses, so that ptxas schedules a slot read where the load it replaces would have been
+__device__ __forceinline__ void lds256(const double2* p, double (&v)[4]) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(p);
+    asm volatile("ld.shared.v2.f64 {%0,%1}, [%4];\n\tld.shared.v2.f64 {%2,%3}, [%4+512];"
+                 : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "r"(a) : "memory");
+}
+__device__ __forceinline__ void sts256(double2* p, const double (&v)[4]) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(p);
+    asm volatile("st.shared.v2.f64 [%0], {%1,%2};\n\tst.shared.v2.f64 [%0+512], {%3,%4};"
+                 :: "r"(a), "d"(v[0]), "d"(v[1]), "d"(v[2]), "d"(v[3]) : "memory");
+}
+
+// dynamic shared memory of a 4-warp block's sibling stack: [slot][warp][R][2][32] 16-byte entries
+constexpr size_t stackBytes(int slots, int R) { return (size_t)slots * 4 * R * 64 * sizeof(double2); }
+// the instances that carry the sibling stack: CP = 4 at the default launch bound of 3 blocks, R <= 4.  ptxas keeps them
+// without a spill and the stack keeps their 3 blocks per SM; elsewhere (other CP, launch bounds 4-6, R = 8) the slot code
+// would cost spills or blocks, so those instances are built without it and ignore the slot bytes
+__host__ __device__ constexpr bool stackBuilt(int CP, int R, int MINB) { return CP == 4 && MINB == 3 && R <= 4; }
+
 template <int CP, int R, bool VIRT>
 struct WarpStage {
     static constexpr int G = 32 / CP, NP = G * R, TABLES = VIRT ? 4 : 2;
@@ -280,7 +309,7 @@ struct WarpStage {
     alignas(16) unsigned char st[TABLES][NP < 16 ? 16 : NP];
 };
 
-template <typename T, int CP, int R, bool VIRT>
+template <typename T, int CP, int R, bool VIRT, bool STACK>
 __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     constexpr int G = 32 / CP, NP = G * R;
     constexpr int PIECE = NP < 16 ? NP : 16;                       // state bytes travel in 4-, 8- or 16-byte pieces
@@ -290,6 +319,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     __shared__ __align__(16) WarpStage<CP, R, VIRT> stages[4][2];
     __shared__ __align__(16) Op4 rings[4][4];
     __shared__ __align__(16) int4 tipRings[4][VIRT ? 4 : 1];
+    extern __shared__ double2 sibStack[];
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));            // volatile: never rematerialised as an S2R inside the loop
     const int wib = threadIdx.x >> 5;
@@ -306,6 +336,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     WarpStage<CP, R, VIRT>* stage = stages[wib];
     Op4* ring = rings[wib];
     int4* tipRing = tipRings[wib];
+    double2* const myStack = sibStack + wib * R * 64 + lane;       // + (slot * 4 * R + r) * 64, halves 32 entries apart
 
     // the gap column (row 4 of every table), once
     for (int q = lane; q < 2 * TABLES * CP * 4; q += 32) {
@@ -325,11 +356,12 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     };
     // what op j reads beyond partials goes to stage j & 1; reads record j from the ring (it has arrived) ONCE -- the fields
     // the compute part needs travel on in registers (4 shared-memory reads per op instead of 20)
-    struct Rec { int dest, c1, c2, sw, sr, flags, pfA, pfB; };
+    struct Rec { int dest, c1, c2, sw, sr, flags, pfA, pfB, slots; };
     auto issueOperands = [&](int j) -> Rec {
         const int4 rec = *reinterpret_cast<const int4*>(&ring[j & 3]);          // dest, c1, c2, m1
         const int4 rec2 = *(reinterpret_cast<const int4*>(&ring[j & 3]) + 1);   // m2, sw, sr, cum
         const int flags = ring[j & 3].pad_;
+        const int slots = STACK ? (int)ring[j & 3].slots : 0xFFFFFF;
         const int2 pf = *reinterpret_cast<const int2*>(&ring[j & 3].pfA);
         const int m2 = rec2.x;
         WarpStage<CP, R, VIRT>& sg = stage[j & 1];
@@ -370,7 +402,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
             if (lane < RECQ + TABLES * SL - 32) statePiece(lane + 32 - RECQ);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
-        return Rec{rec.x, rec.y, rec.z, rec2.y, rec2.z, flags, pf.x, pf.y};
+        return Rec{rec.x, rec.y, rec.z, rec2.y, rec2.z, flags, pf.x, pf.y, slots};
     };
     // prologue: records k0 (and k0+1 through issueOperands), then the operands of k0
     if (lane < RECQ) fetchRecord(range.x);
@@ -420,6 +452,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
                 const double e[4] = {e01.x, e01.y, e23.x, e23.y};
                 const bool fromRegisters = ch == 0 && (cur.flags & 2) != 0;
                 const bool virt = VIRT && (cur.flags & (4 << ch)) != 0;
+                const int src = STACK ? (cur.slots >> (8 * ch)) & 0xFF : 0xFF;
                 const T* xg = static_cast<const T*>(A.partials) + (size_t)child * A.stride + off0;
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
@@ -437,6 +470,8 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
                         const double2 bHi = *reinterpret_cast<const double2*>(&sg.mat[TABLES - 2 + ch][10 * CP + eB]);
                         x[0] = aLo.x * bLo.x; x[1] = aLo.y * bLo.y; x[2] = aHi.x * bHi.x; x[3] = aHi.y * bHi.y;
                         roundCell<T>(x);
+                    } else if (STACK && src != 0xFF) {                  // a sibling this thread parked earlier
+                        lds256(myStack + (src * 4 * R + r) * 64, x);
                     } else {
                         loadCell(xg + (size_t)r * G * 4, x);
                     }
@@ -452,6 +487,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
             }
         }
         T* dg = static_cast<T*>(A.partials) + (size_t)cur.dest * A.stride + off0;
+        const int dst = STACK ? (cur.slots >> 16) & 0xFF : 0xFF;
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             const int p = p0 + r * G;
@@ -473,6 +509,7 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
             }
             roundCell<T>(d[r]);
             if (catValid) storeCell(dg + (size_t)r * G * 4, d[r]);
+            if (STACK && dst != 0xFF) sts256(myStack + (dst * 4 * R + r) * 64, d[r]);
         }
         asm volatile("cp.async.wait_group 0;" ::: "memory");      // op k+1's operands and record k+2 have landed
         __syncwarp();
@@ -482,42 +519,67 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4p(const WalkArgs A) {
-    walk4pBody<double, CP, R, false>(A);
+    walk4pBody<double, CP, R, false, stackBuilt(CP, R, MINB)>(A);
 }
 
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4ps(const WalkArgs A) {
-    walk4pBody<float, CP, R, false>(A);
+    walk4pBody<float, CP, R, false, stackBuilt(CP, R, MINB)>(A);
 }
 
 // lists that read virtual cherries: twice the tip tables per warp stage
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4pv(const WalkArgs A) {
-    walk4pBody<double, CP, R, true>(A);
+    walk4pBody<double, CP, R, true, stackBuilt(CP, R, MINB)>(A);
 }
 
 template <int CP, int R, int MINB>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4pvs(const WalkArgs A) {
-    walk4pBody<float, CP, R, true>(A);
+    walk4pBody<float, CP, R, true, stackBuilt(CP, R, MINB)>(A);
+}
+
+// stackSlots: the sibling stack of the phase (dynamic shared memory; 0 on instances built without it).  The kernel's
+// limit is set once per device to the deepest stack it can get (kStackSlots slots), never lowered: instances on other host
+// threads launch the same kernel with other depths.  No carveout preference: the driver sizes shared memory per launch, so
+// launches without a stack keep the larger L1.
+template <auto KERNEL, int CP, int R, int MINB>
+cudaError_t launchStaged(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
+    const size_t smem = stackBuilt(CP, R, MINB) ? stackBytes(stackSlots, R) : 0;
+    if (smem > 0) {
+        static std::atomic<unsigned long long> limitSet{0};             // one bit per device
+        const unsigned long long bit = 1ull << (in->device & 63);
+        if (!(limitSet.load() & bit)) {
+            cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)stackBytes(kStackSlots, R));
+            if (e != cudaSuccess) return e;
+            limitSet.fetch_or(bit);
+        }
+    }
+    if (in->debugLog) {
+        const auto kernel = KERNEL;
+        int blocks = 0;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kernel, 128, smem);
+        fprintf(stderr, "[b200-beagle] staged walk: %zu B sibling stack per block, %d blocks per SM\n", smem, blocks);
+    }
+    KERNEL<<<grid, 128, smem, in->stream>>>(A);
+    return cudaGetLastError();
 }
 
 template <typename T, int CP, int R, int MINB>
-cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid) {
-    if constexpr (sizeof(T) == 4) k_walk4ps<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
-    else k_walk4p<CP, R, MINB><<<grid, 128, 0, in->stream>>>(A);
-    return cudaGetLastError();
+cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
+    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4ps<CP, R, MINB>, CP, R, MINB>(in, A, grid, stackSlots);
+    else return launchStaged<k_walk4p<CP, R, MINB>, CP, R, MINB>(in, A, grid, stackSlots);
 }
 
 // one launch bound only (B200_WALK_MINB does not apply): with 3 blocks ptxas keeps the doubled staging in registers without
 // a spill at every R the virtual kernel serves (R = 8 phases keep their cherries, see walk4pServes)
 template <typename T, int CP, int R>
-cudaError_t launchPV(Instance* in, const WalkArgs& A, dim3 grid) {
-    if constexpr (sizeof(T) == 4) k_walk4pvs<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
-    else k_walk4pv<CP, R, 3><<<grid, 128, 0, in->stream>>>(A);
-    return cudaGetLastError();
+cudaError_t launchPV(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
+    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4pvs<CP, R, 3>, CP, R, 3>(in, A, grid, stackSlots);
+    else return launchStaged<k_walk4pv<CP, R, 3>, CP, R, 3>(in, A, grid, stackSlots);
 }
 
 // recipe rows [buffer][2][16 * CP] of the virtual cherries a list produces: items (buffer, m1, m2, -)
@@ -589,8 +651,9 @@ bool stagedWalk(const Instance* in, int R, bool aligned) {
     return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4 && (R == 1 ? in->thinTipMode : in->tipMode) == 3;
 }
 
+// stackSlots: slots per warp of the phase's sibling stack (0 = none)
 template <typename T, int CP, int R>
-cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
+cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt, int stackSlots) {
     constexpr int G = 32 / CP;
     constexpr int TIPD = CP <= 8 ? 2 : 0;
     const int warps = (maxWindow + G * R - 1) / (G * R);
@@ -599,17 +662,17 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
         if (stagedWalk(in, R, aligned)) {                          // per-warp asynchronous operand staging (k_walk4p)
             if (virt) {
                 if constexpr (R == 8) return cudaErrorInvalidValue;
-                else return launchPV<T, CP, R>(in, A, grid);
+                else return launchPV<T, CP, R>(in, A, grid, stackSlots);
             }
             if constexpr (CP == 4) {
                 // a launch bound of 3 blocks lets ptxas keep its registers without a spill and 4 blocks still fit -- the
                 // fastest setting where it was swept, unless B200_WALK_MINB says otherwise
                 const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;
-                if (minb >= 6) return launchP<T, CP, R, 6>(in, A, grid);
-                if (minb == 5) return launchP<T, CP, R, 5>(in, A, grid);
-                if (minb == 3) return launchP<T, CP, R, 3>(in, A, grid);
+                if (minb >= 6) return launchP<T, CP, R, 6>(in, A, grid, stackSlots);
+                if (minb == 5) return launchP<T, CP, R, 5>(in, A, grid, stackSlots);
+                if (minb == 3) return launchP<T, CP, R, 3>(in, A, grid, stackSlots);
             }
-            return launchP<T, CP, R, 4>(in, A, grid);
+            return launchP<T, CP, R, 4>(in, A, grid, stackSlots);
         }
     }
     if (virt) return cudaErrorInvalidValue;                        // only k_walk4p reads virtual cherries
@@ -633,17 +696,22 @@ cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool al
 }
 
 template <typename T, int CP>
-cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt) {
+cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt, int stackSlots) {
     const int R = phaseR(in, nSubs, maxWindow);
-    if (R == 1) return launchR<T, CP, 1>(in, A, nSubs, maxWindow, aligned, virt);
+    if (R == 1) return launchR<T, CP, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     if constexpr (CP == 4) {
-        if (R == 8) return launchR<T, CP, 8>(in, A, nSubs, maxWindow, aligned, virt);
-        if (R == 2) return launchR<T, CP, 2>(in, A, nSubs, maxWindow, aligned, virt);
+        if (R == 8) return launchR<T, CP, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+        if (R == 2) return launchR<T, CP, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     }
-    return launchR<T, CP, 4>(in, A, nSubs, maxWindow, aligned, virt);
+    return launchR<T, CP, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
 }
 
 }  // namespace
+
+bool walkStackBuilt(const Instance* in) {
+    const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;     // the launch bound launchR picks for k_walk4p
+    return stackBuilt(in->matCP, in->walkR == 8 ? 8 : 4, minb);
+}
 
 bool walk4pServes(const Instance* in, int nSubs, int maxWindow) {
     if (in->matCP == 0) return false;
@@ -653,7 +721,7 @@ bool walk4pServes(const Instance* in, int nSubs, int maxWindow) {
 
 // eigen: [V (16, row-major Evec[i][k]) | V^-1 (16, Ievc[k][j])], padded to 4 x 4 with zeros
 cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
-                         const double* eigen, const int4* dVirtTips) {
+                         const double* eigen, const int4* dVirtTips, int stackSlots) {
     const bool virt = dVirtTips != nullptr;
     if (nSubs <= 0) return cudaSuccess;
     WalkArgs A;
@@ -668,21 +736,21 @@ cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int n
     for (int q = 0; q < 16; ++q) { A.V[q] = eigen[q]; A.Vi[q] = eigen[16 + q]; }
     if (in->single) {                                // CP <= 8 only: single instances have C <= 8
         switch (in->matCP) {
-            case 1: return launchCP<float, 1>(in, A, nSubs, maxWindow, aligned, virt);
-            case 2: return launchCP<float, 2>(in, A, nSubs, maxWindow, aligned, virt);
-            case 8: return launchCP<float, 8>(in, A, nSubs, maxWindow, aligned, virt);
-            default: return launchCP<float, 4>(in, A, nSubs, maxWindow, aligned, virt);
+            case 1: return launchCP<float, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+            case 2: return launchCP<float, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+            case 8: return launchCP<float, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+            default: return launchCP<float, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         }
     }
     switch (in->matCP) {
 #ifndef B200_W4E_QUICK
-        case 1: return launchCP<double, 1>(in, A, nSubs, maxWindow, aligned, virt);
-        case 2: return launchCP<double, 2>(in, A, nSubs, maxWindow, aligned, virt);
-        case 8: return launchCP<double, 8>(in, A, nSubs, maxWindow, aligned, virt);
-        case 16: return launchCP<double, 16>(in, A, nSubs, maxWindow, aligned, virt);
-        case 32: return launchCP<double, 32>(in, A, nSubs, maxWindow, aligned, virt);
+        case 1: return launchCP<double, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+        case 2: return launchCP<double, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+        case 8: return launchCP<double, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+        case 16: return launchCP<double, 16>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+        case 32: return launchCP<double, 32>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
 #endif
-        default: return launchCP<double, 4>(in, A, nSubs, maxWindow, aligned, virt);
+        default: return launchCP<double, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     }
 }
 

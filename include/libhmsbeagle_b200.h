@@ -379,6 +379,16 @@ BEAGLE_DLLEXPORT int b200DebugPlan(const int* operations, int operationCount, in
                                    int minT, int smallRemainder, int preOrder, int* outOrder, int* outSubs,
                                    int* outPhaseStart, int* outCounts);
 
+/* Host-logic test hook (no CUDA): the post-order plan of a 7-int-per-op list (as b200DebugPlan with fixedT = 0), the
+ * register forwarding between consecutive ops of a walk and the sibling-stack slots of the staged eigen walk.  Buffers
+ * below tipCount are compact tips.  outRecords[5 * position] = {dest, child 1, child 2, flags, slots} of the op record
+ * (a tip child is -(buffer + 1); flags bit 1 = child 1 is taken from registers; slots = byte 0 / 1 the slot child 1 / 2
+ * is read from, byte 2 the slot the result is kept in, 0xFF = none); outSubs, outPhaseStart as in b200DebugPlan;
+ * outCounts = {subtrees, phases, children read from a slot, internal children read from memory, deepest slot used}. */
+BEAGLE_DLLEXPORT int b200DebugStackSlots(const int* operations, int operationCount, int bufferCount, int tipCount,
+                                         int wantSubs, int minT, int smallRemainder, int* outRecords, int* outSubs,
+                                         int* outPhaseStart, int* outCounts);
+
 #ifdef __cplusplus
 }
 #endif
