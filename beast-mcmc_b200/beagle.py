@@ -165,6 +165,8 @@ _SIGNATURES = {
     "b200SetKernelTiming": ([_I, _I], _I),
     "b200GetKernelTiming": ([_I, _I, _DP, C.POINTER(C.c_long)], _I),
     "b200CompressSitePatterns": ([_I, _I, _I, _IP, _DP, _IP, _IP, _DP, _IP], _I),
+    "b200SampleAncestralStates": ([_I, _IP, _IP, _IP, _I, _I, _I, _I, C.c_ulonglong, C.c_ulonglong, _IP, _IP], _I),
+    "b200DebugAncestralRows": ([_IP, _IP, _IP, _I, _I, _I], _I),
     "b200GetSourceHash": ([], C.c_char_p),
     "b200GetFusedLaunches": ([_I], _L),
     "b200RootLogLikelihoodsByPartitionDevice": ([_I, _IP, _IP, _IP, _IP, _IP, _I, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)], _I),
@@ -457,6 +459,21 @@ class BeagleJNIImpl(Beagle):
         self._check("b200GetKernelTiming", self._lib.b200GetKernelTiming(self.instance, which, C.byref(ms), C.byref(n)))
         return ms.value, n.value
 
+    def sampleAncestralStates(self, nodeBuffers, parentRows, matrixIndices, rootBuffer, categoryWeightsIndex,
+                              stateFrequenciesIndex, seed, drawIndex):
+        """One joint draw of ancestral states per pattern (b200SampleAncestralStates): rows in pre-order, row 0 the root ->
+        (states int32 [rows][patternCount], categories int32 [patternCount])."""
+        nb, pr, mi = _ip(nodeBuffers), _ip(parentRows), _ip(matrixIndices)
+        count = len(nb[0])
+        assert len(pr[0]) == count and len(mi[0]) == count
+        states = np.zeros((count, self.patternCount), dtype=np.int32)
+        cats = np.zeros(self.patternCount, dtype=np.int32)
+        self._check("sampleAncestralStates",
+                    self._lib.b200SampleAncestralStates(self.instance, nb[1], pr[1], mi[1], count, rootBuffer,
+                                                        categoryWeightsIndex, stateFrequenciesIndex, seed, drawIndex,
+                                                        states.ctypes.data_as(_IP), cats.ctypes.data_as(_IP)))
+        return states, cats
+
 
 class BeagleFactory:
     @staticmethod
@@ -496,3 +513,10 @@ def compressSitePatterns(states, siteWeights=None, resource: int = 1):
         raise BeagleException("compressSitePatterns", rc)
     P = n.value
     return pats[:taxa * P].reshape(taxa, P).copy(), w[:P].copy(), idx[:sites].copy()
+
+
+def checkAncestralRows(nodeBuffers, parentRows, matrixIndices, bufferCount, matrixCount) -> int:
+    """The row rules of b200SampleAncestralStates on the host (b200DebugAncestralRows): 0 or OUT_OF_RANGE_ERROR."""
+    lib = load_library()
+    nb, pr, mi = _ip(nodeBuffers), _ip(parentRows), _ip(matrixIndices)
+    return lib.b200DebugAncestralRows(nb[1], pr[1], mi[1], len(nb[0]), bufferCount, matrixCount)

@@ -23,7 +23,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-ENGINE_UNITS = ("api.cu", "kernels.cu", "walk4e.cu", "incr.cu", "multi.cu", "patterns.cu")
+ENGINE_UNITS = ("api.cu", "kernels.cu", "walk4e.cu", "incr.cu", "multi.cu", "patterns.cu", "ancestral.cu")
 ENGINE_HEADERS = (os.path.join(CSRC, "engine.h"), os.path.join(CSRC, "walk4.cuh"), os.path.join(CSRC, "multi.h"),
                   os.path.join(ROOT, "include", "libhmsbeagle_b200.h"))
 

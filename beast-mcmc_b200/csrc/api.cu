@@ -2444,6 +2444,82 @@ int b200DebugStackSlots(const int* operations, int operationCount, int bufferCou
     return BEAGLE_SUCCESS;
 }
 
+// ---- joint ancestral-state sampling (ancestral.cu) ---------------------------------------------------------------------
+// the row rules, no CUDA calls: row 0 is the root (parent -1; its node buffer and matrix are not read), every later row
+// names a buffer, a parent row before it and a matrix buffer
+int b200DebugAncestralRows(const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                           int bufferCount, int matrixCount) {
+    if (count < 1 || nodeBuffers == nullptr || parentRows == nullptr || matrixIndices == nullptr || parentRows[0] != -1)
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    for (int r = 1; r < count; ++r)
+        if (!validRange(nodeBuffers[r], bufferCount) || !validRange(parentRows[r], r) || !validRange(matrixIndices[r], matrixCount))
+            return BEAGLE_ERROR_OUT_OF_RANGE;
+    return BEAGLE_SUCCESS;
+}
+
+int b200SampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                              int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex, unsigned long long seed,
+                              unsigned long long drawIndex, int* outStates, int* outCategories) {
+    SH(instance, shSampleAncestralStates(sh, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex,
+                                         stateFrequenciesIndex, seed, drawIndex, outStates, outCategories));
+    return sampleAncestralStates(instance, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex,
+                                 stateFrequenciesIndex, seed, drawIndex, 0, outStates, outCategories);
+}
+
+}  // extern "C"
+
+int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                int count, int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex,
+                                unsigned long long seed, unsigned long long drawIndex, int patternOffset, int* outStates,
+                                int* outCategories) {
+    GET_INSTANCE_LAZY(in, instance);
+    // everything is checked before anything is launched, the deferred work of earlier calls included
+    if (outStates == nullptr || outCategories == nullptr ||
+        b200DebugAncestralRows(nodeBuffers, parentRows, matrixIndices, count, in->nBuffers, in->nMatrices) != BEAGLE_SUCCESS ||
+        !validRange(rootBuffer, in->nBuffers) || !validRange(categoryWeightsIndex, in->nSets) ||
+        !validRange(stateFrequenciesIndex, in->nSets))
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    // a buffer must hold data: partials (a deferred list has already assigned its destinations) or compact states
+    auto holdsData = [&](int b) { return in->partials[b] != nullptr || in->states32[b] != nullptr; };
+    if (!holdsData(rootBuffer)) return BEAGLE_ERROR_OUT_OF_RANGE;
+    for (int r = 1; r < count; ++r) if (!holdsData(nodeBuffers[r])) return BEAGLE_ERROR_OUT_OF_RANGE;
+    if (!in->pendingMats.empty() || !in->pendingOps.empty()) { const int rc = flushPending(in); if (rc != BEAGLE_SUCCESS) return rc; }
+    std::vector<int> bufs(nodeBuffers, nodeBuffers + count);
+    bufs[0] = rootBuffer;
+    CUDA_OK(storeCherries(in, bufs.data(), count));       // virtual cherries have no stored partials until asked for them
+    std::vector<int4> rows(count);
+    for (int r = 0; r < count; ++r) {
+        const int b = bufs[r];
+        rows[r] = make_int4(in->states32[b] != nullptr ? -(b + 1) : in->slotOf[b], r == 0 ? -1 : parentRows[r],
+                            r == 0 ? 0 : matrixIndices[r], 0);
+    }
+    const size_t outInts = (size_t)(count + 1) * in->P;          // [categories P | states count x P]: ONE D2H copy
+    CUDA_OK(ensureScratch(in, (outInts + 1) / 2));
+    const int4* dRows = static_cast<const int4*>(stage(in, rows.data(), sizeof(int4) * count));
+    if (dRows == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
+    AncestralArgs a;
+    a.rows = dRows; a.count = count; a.P = in->P; a.Ppad = in->Ppad; a.S = in->S; a.Sp = in->Sp; a.C = in->C; a.CP = in->matCP;
+    a.pOffset = patternOffset;
+    a.partials = in->partialsBase; a.stride = in->partialsElems;
+    a.states8 = in->states8Base; a.states32 = in->states32Base;
+    a.mats = in->dMat; a.matStride = in->matStride;
+    a.weights = in->dWeights + (size_t)categoryWeightsIndex * in->C;
+    a.freqs = in->dFreqs + (size_t)stateFrequenciesIndex * in->Sp;
+    a.seed = seed; a.drawIndex = drawIndex;
+    int* dOut = reinterpret_cast<int*>(in->dScratch);
+    a.outCategories = dOut;
+    a.outStates = dOut + in->P;
+    CUDA_OK(launchAncestral(in, a));
+    std::vector<int> host(outInts);
+    CUDA_OK(cudaMemcpyAsync(host.data(), dOut, sizeof(int) * outInts, cudaMemcpyDeviceToHost, in->stream));
+    CUDA_OK(cudaStreamSynchronize(in->stream));
+    memcpy(outCategories, host.data(), sizeof(int) * in->P);
+    memcpy(outStates, host.data() + in->P, sizeof(int) * (size_t)count * in->P);
+    return BEAGLE_SUCCESS;
+}
+
+extern "C" {
+
 // ---- engine extensions ------------------------------------------------------------------------
 int b200SetKernelTiming(int instance, int enable) {
     SH(instance, shBroadcast(sh, [&](int c) { return b200SetKernelTiming(c, enable); }));

@@ -318,4 +318,27 @@ cudaError_t launchScaleAccumulate(Instance* in, const int* dIdx, int count, doub
                                   int pBegin, int pEnd);
 cudaError_t launchRescalePartialsForGet(Instance* in, double* tmp, const double* cum);
 
+// ---- joint ancestral-state sampling (ancestral.cu) ----------------------------------------------------------------------
+struct AncestralArgs {
+    const int4* rows;             // [row] = (partials slot, or -(tip + 1) for a compact tip; parent row; matrix buffer; 0)
+    int count, P, Ppad, S, Sp, C, CP;
+    int pOffset;                  // global index of pattern 0 (a shard's first pattern): the Philox counter carries it
+    const void* partials;         // slab base (float on a PRECISION_SINGLE instance)
+    size_t stride;                // elements per slot
+    const uint8_t* states8;       // [tip][Ppad] (4-state matrix layout)
+    const int* states32;          // [tip][Ppad] (generic layout)
+    const double* mats;
+    size_t matStride;
+    const double* weights;        // [C] of the chosen set
+    const double* freqs;          // [Sp] of the chosen set
+    unsigned long long seed, drawIndex;
+    int* outStates;               // [count][P]
+    int* outCategories;           // [P]
+};
+cudaError_t launchAncestral(Instance* in, const AncestralArgs& args);
+// api.cu: b200SampleAncestralStates on one single-device instance; patternOffset = global index of its first pattern
+int sampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                          int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex, unsigned long long seed,
+                          unsigned long long drawIndex, int patternOffset, int* outStates, int* outCategories);
+
 }  // namespace b200

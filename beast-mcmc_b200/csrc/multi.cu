@@ -377,6 +377,30 @@ int shEdgeDerivatives(Sharded* sh, const int* post, const int* pre, const int* d
     return BEAGLE_SUCCESS;
 }
 
+// every shard samples its block with the GLOBAL pattern index in the Philox counter: the draws equal the unsharded instance's
+int shSampleAncestralStates(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                            int rootBuffer, int wIdx, int fIdx, unsigned long long seed, unsigned long long drawIndex,
+                            int* outStates, int* outCategories) {
+    if (count < 1 || outStates == nullptr || outCategories == nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
+    std::vector<std::vector<int>> states(sh->g), cats(sh->g);
+    const int rc = sh->pool->run([&](int k) {
+        if (sh->count[k] == 0) return 0;
+        states[k].resize((size_t)count * sh->count[k]);
+        cats[k].resize(sh->count[k]);
+        return sampleAncestralStates(sh->child[k], nodeBuffers, parentRows, matrixIndices, count, rootBuffer, wIdx, fIdx, seed,
+                                     drawIndex, sh->begin[k], states[k].data(), cats[k].data());
+    });
+    if (rc != 0) return rc;
+    for (int k = 0; k < sh->g; ++k) {
+        if (sh->count[k] == 0) continue;
+        memcpy(outCategories + sh->begin[k], cats[k].data(), sizeof(int) * sh->count[k]);
+        for (int r = 0; r < count; ++r)
+            memcpy(outStates + (size_t)r * sh->P + sh->begin[k], states[k].data() + (size_t)r * sh->count[k],
+                   sizeof(int) * sh->count[k]);
+    }
+    return BEAGLE_SUCCESS;
+}
+
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq) {
     if (outSumSq != nullptr) return BEAGLE_ERROR_NO_IMPLEMENTATION;

@@ -14,6 +14,9 @@ int shGetPerPattern(Sharded* sh, double* out, const std::function<int(int, doubl
 int shRoot(Sharded* sh, const int* bufferIndices, const int* wIdx, const int* fIdx, const int* cumIdx, int count, double* out);
 int shEdgeDerivatives(Sharded* sh, const int* post, const int* pre, const int* dmat, const int* wIdx, int count, double* outPer,
                       double* outSum, double* outSumSq);
+int shSampleAncestralStates(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                            int rootBuffer, int wIdx, int fIdx, unsigned long long seed, unsigned long long drawIndex,
+                            int* outStates, int* outCategories);
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq);
 }  // namespace b200

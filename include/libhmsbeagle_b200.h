@@ -370,6 +370,34 @@ BEAGLE_DLLEXPORT int b200CompressSitePatterns(int resourceNumber, int taxonCount
                                               const double* inSiteWeights, int* outSitePatternIndices, int* outPatterns,
                                               double* outWeights, int* outPatternCount);
 
+/* Joint ancestral states on the device: per pattern p ONE draw of (rate category, state of every listed node) from the
+ * exact joint posterior given the data, the post-order partials the instance holds and its transition matrices (what
+ * AncestralStateBeagleTreeLikelihood draws in Java from getPartials / getTransitionMatrix; DESIGN.md section 7).
+ * Rows in pre-order: row 0 is the root (parentRows[0] = -1; nodeBuffers[0] and matrixIndices[0] are not read), every other
+ * row r names its node's post-order buffer nodeBuffers[r], its parent row parentRows[r] < r and the matrix buffer of the
+ * branch above it matrixIndices[r].
+ *   root : (c, i) with probability proportional to w_c * pi_i * Lroot_c[p][i]   (rootBuffer, categoryWeightsIndex,
+ *          stateFrequenciesIndex)
+ *   row r: j given the parent row's state i and the root's category c, proportional to P_c[i][j] * L_r,c[p][j]; a compact
+ *          tip keeps its observed state, a gap / unknown state draws proportional to P_c[i][j]; tips given as partials and
+ *          internal buffers use their partials
+ * Each draw is an inverse CDF over the items in index order ((c, i) category-major at the root) with fp64 cumulative sums;
+ * the uniform is (x >> 11) * 2^-53, x = the first output word of Philox4x64-10 (numpy.random.Philox) with key (seed, 0) and
+ * counter (drawIndex, global pattern index, row, 0), so a draw depends on neither the launch geometry nor the sharding.
+ * If no cumulative sum exceeds u * total (all weights zero: data impossible under the model) the last item of positive
+ * weight is taken, else item 0.  Rescale factors cancel in every conditional: scale buffers are not inputs.
+ * outStates[row * patternCount + p] (int, capacity count * patternCount), outCategories[p].  Returns
+ * BEAGLE_ERROR_OUT_OF_RANGE, launching nothing, for a parent row not before its child, an index out of range or a buffer
+ * that holds neither partials nor tip states. */
+BEAGLE_DLLEXPORT int b200SampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows,
+                                               const int* matrixIndices, int count, int rootBuffer, int categoryWeightsIndex,
+                                               int stateFrequenciesIndex, unsigned long long seed,
+                                               unsigned long long drawIndex, int* outStates, int* outCategories);
+/* Host-logic test hook (no CUDA): the row rules of b200SampleAncestralStates for an instance with bufferCount buffers and
+ * matrixCount matrices; 0 or BEAGLE_ERROR_OUT_OF_RANGE. */
+BEAGLE_DLLEXPORT int b200DebugAncestralRows(const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                                            int bufferCount, int matrixCount);
+
 /* Host-logic test hook (no CUDA): the engine's execution plan for a 7-int-per-op list.  outOrder[n] = execution
  * position -> caller index; outSubs = (begin,end) position pairs of the independent subtree walks, grouped by phase;
  * outPhaseStart = index of each phase's first subtree (phases+1 entries); outCounts = {subtrees, phases}.
