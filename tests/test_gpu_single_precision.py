@@ -339,8 +339,8 @@ def test_by_partition_route(scheme):
 
 
 # ---- 7. gradients --------------------------------------------------------------------------------------------------------
-def _gradient_pair(S, seed):
-    tree, pats, model, site = H.synthetic_case(30, 600, categories=4, seed=seed, stateCount=S)
+def _gradient_pair(S, seed, C=4):
+    tree, pats, model, site = H.synthetic_case(30, 600, categories=C, seed=seed, stateCount=S)
     out = []
     for factory, res, pref in ((GPU, [1, 0], SINGLE), (H.oracle_factory(), None, 0)):
         d = _delegate(tree, pats, model, site, factory, res, S_.NONE, pref, usePreOrder=True)
@@ -350,8 +350,9 @@ def _gradient_pair(S, seed):
     return tree, pats, model, out[0], out[1]
 
 
+@pytest.mark.parametrize("C", [4, 1, 8])
 @pytest.mark.parametrize("S", [2, 4])
-def test_edge_derivatives_bound(S):
+def test_edge_derivatives_bound(S, C):
     """Per pattern and edge, d_p = num_p / L_p with num_p = sum_c w_c sum_jk pre_cj D_cjk post_ck and
     L_p = sum_c w_c sum_j pre_cj post_cj.  Every pre and post value passed through at most N stored fp32 buffers, so it
     carries a factor (1 + e) with |e| <= 1.001 N u (N = all pre- and post-order buffers; n u << 1 keeps the 1.001).  A term
@@ -360,7 +361,7 @@ def test_edge_derivatives_bound(S):
         |dd_p| <= |dnum| / L + |d_p| |dL| / L <= 1.001 u (2N A_p/L_p + 2N |d_p|) <= 1.001 u (3N A_p/L_p + N |d_p|)
     as |d_p| <= A_p / L_p.  1e-9 A_p/L_p covers the fp64 differences from the oracle.  A_p comes from the oracle's
     partials."""
-    tree, pats, model, g, o = _gradient_pair(S, 91 + S)
+    tree, pats, model, g, o = _gradient_pair(S, 91 + S, C)
     nodes = [n for n in range(tree.nodeCount) if n != tree.root]
     N = (tree.nodeCount - tree.tipCount) + tree.nodeCount
     dg, do = tdl.DiscreteTraitBranchRateDelegate(tree, g, model), tdl.DiscreteTraitBranchRateDelegate(tree, o, model)
@@ -388,12 +389,13 @@ def test_edge_derivatives_bound(S):
         assert np.all(np.abs(d_g - d_o) <= bound), (node, np.max(np.abs(d_g - d_o) / bound))
 
 
+@pytest.mark.parametrize("C", [4, 1, 8])
 @pytest.mark.parametrize("S", [2, 4])
-def test_cross_products_bound(S):
+def test_cross_products_bound(S, C):
     """out[i][j] = sum_e t_e sum_p w_p (sum_c w_c r_c pre_ci post_cj) / L_p: every term is non-negative, the numerator carries
     two factors (1 + e) and L_p two more, |e| <= 1.001 N u, so each entry is within 1.001 * 4 N u of the oracle's
     (relative), plus 1e-9 for the fp64 differences."""
-    tree, pats, model, g, o = _gradient_pair(S, 95 + S)
+    tree, pats, model, g, o = _gradient_pair(S, 95 + S, C)
     N = (tree.nodeCount - tree.tipCount) + tree.nodeCount
     xg = tdl.SubstitutionModelCrossProductDelegate(tree, g, model).getCrossProducts()
     xo = tdl.SubstitutionModelCrossProductDelegate(tree, o, model).getCrossProducts()

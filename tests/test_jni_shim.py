@@ -17,13 +17,15 @@ TYPE2DESC = {"jint": "I", "jlong": "J", "jdouble": "D", "jintArray": "[I", "jdou
 
 
 @pytest.fixture(scope="module")
-def jni():
+def jni(tmp_path_factory):
     build.build_engine()
     lib = build.build_jni()
-    exe = os.path.join(ROOT, "tests", "jni_fake", "fake_jvm")
-    src = exe + ".cpp"
-    if not os.path.exists(exe) or os.path.getmtime(exe) < os.path.getmtime(src):
-        subprocess.run(["g++", "-O1", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-o", exe, src, "-ldl"], check=True)
+    src = os.path.join(ROOT, "tests", "jni_fake", "fake_jvm.cpp")
+    # built into this session's own temporary directory: the checkout may be read-only or shared with another run
+    exe = str(tmp_path_factory.mktemp("jni_fake") / "fake_jvm")
+    r = subprocess.run(["g++", "-O1", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-o", exe, src, "-ldl"],
+                       capture_output=True, text=True)
+    assert r.returncode == 0, r.stdout + r.stderr
     return lib, exe
 
 

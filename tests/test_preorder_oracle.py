@@ -52,7 +52,9 @@ def test_oracle_preorder_identity_and_gradient(states, cats):
 # ---- the CUDA engine through the C ABI ---------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("states,cats,tips,patterns", [(4, 1, 10, 70), (4, 4, 40, 300), (4, 5, 16, 100), (20, 2, 12, 90),
-                                                       (61, 1, 8, 64), (7, 3, 9, 50)])
+                                                       (61, 1, 8, 64), (7, 3, 9, 50), (4, 2, 10, 97), (4, 8, 12, 301),
+                                                       (4, 13, 9, 61), (4, 24, 8, 45), (4, 40, 8, 33), (9, 2, 8, 70),
+                                                       (30, 2, 8, 70)])
 def test_gpu_preorder_matches_oracle_and_finite_differences(states, cats, tips, patterns):
     from beast_mcmc_b200 import beagle
     tree, pats, model, site = H.synthetic_case(tips, patterns, cats, seed=5 + states + tips, stateCount=states)
@@ -134,7 +136,8 @@ def test_oracle_cross_products_contract_to_scale_derivative(states, cats):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("states,cats,tips,patterns", [(4, 1, 10, 70), (4, 4, 40, 700), (4, 5, 16, 100), (20, 2, 12, 90),
-                                                       (61, 2, 8, 75), (7, 3, 9, 50), (70, 1, 5, 40)])
+                                                       (61, 2, 8, 75), (7, 3, 9, 50), (70, 1, 5, 40), (4, 13, 10, 300),
+                                                       (16, 2, 8, 70), (30, 2, 8, 70), (3, 4, 9, 80), (40, 2, 6, 40)])
 def test_gpu_cross_products_match_oracle(states, cats, tips, patterns):
     from beast_mcmc_b200 import beagle
     tree, pats, model, site = H.synthetic_case(tips, patterns, cats, seed=3 + states + tips, stateCount=states)
