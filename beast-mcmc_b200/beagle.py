@@ -167,6 +167,8 @@ _SIGNATURES = {
     "b200CompressSitePatterns": ([_I, _I, _I, _IP, _DP, _IP, _IP, _DP, _IP], _I),
     "b200SampleAncestralStates": ([_I, _IP, _IP, _IP, _I, _I, _I, _I, C.c_ulonglong, C.c_ulonglong, _IP, _IP], _I),
     "b200DebugAncestralRows": ([_IP, _IP, _IP, _I, _I, _I], _I),
+    "b200SampleMarkovJumps": ([_I, _IP, _IP, _IP, _DP, _I, _I, _I, _I, _I, _I, _DP, _I, C.c_ulonglong, C.c_ulonglong, _IP, _IP,
+                               _DP, _DP], _I),
     "b200GetSourceHash": ([], C.c_char_p),
     "b200GetFusedLaunches": ([_I], _L),
     "b200RootLogLikelihoodsByPartitionDevice": ([_I, _IP, _IP, _IP, _IP, _IP, _I, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)], _I),
@@ -473,6 +475,32 @@ class BeagleJNIImpl(Beagle):
                                                         categoryWeightsIndex, stateFrequenciesIndex, seed, drawIndex,
                                                         states.ctypes.data_as(_IP), cats.ctypes.data_as(_IP)))
         return states, cats
+
+    def sampleMarkovJumps(self, nodeBuffers, parentRows, matrixIndices, edgeLengths, rootBuffer, categoryWeightsIndex,
+                          stateFrequenciesIndex, eigenIndex, categoryRatesIndex, registerMatrices, seed, drawIndex,
+                          states=True, categories=True, branchCounts=True, patternCounts=True):
+        """Markov-jump counts / rewards conditioned on one joint ancestral draw (b200SampleMarkovJumps): rows as in
+        sampleAncestralStates, edgeLengths [rows], registerMatrices [registers][S][S] -> (states int32 [rows][patternCount],
+        categories int32 [patternCount], branchCounts [registers][rows], patternCounts [registers][patternCount]); an output
+        switched off by its flag is None and not copied back."""
+        nb, pr, mi = _ip(nodeBuffers), _ip(parentRows), _ip(matrixIndices)
+        count = len(nb[0])
+        assert len(pr[0]) == count and len(mi[0]) == count
+        lengths = _dp(np.asarray(edgeLengths, dtype=np.float64).reshape(count))
+        regs = np.ascontiguousarray(registerMatrices, dtype=np.float64)
+        G = regs.shape[0] if regs.ndim == 3 else 1
+        regs = _dp(regs.reshape(-1))
+        outs = (np.zeros((count, self.patternCount), dtype=np.int32) if states else None,
+                np.zeros(self.patternCount, dtype=np.int32) if categories else None,
+                np.zeros((G, count)) if branchCounts else None,
+                np.zeros((G, self.patternCount)) if patternCounts else None)
+        ptr = lambda a, t: None if a is None else a.ctypes.data_as(t)
+        self._check("sampleMarkovJumps",
+                    self._lib.b200SampleMarkovJumps(self.instance, nb[1], pr[1], mi[1], lengths[1], count, rootBuffer,
+                                                    categoryWeightsIndex, stateFrequenciesIndex, eigenIndex,
+                                                    categoryRatesIndex, regs[1], G, seed, drawIndex, ptr(outs[0], _IP),
+                                                    ptr(outs[1], _IP), ptr(outs[2], _DP), ptr(outs[3], _DP)))
+        return outs
 
 
 class BeagleFactory:

@@ -15,7 +15,14 @@
 // c-major at the root) with fp64 cumulative sums: the first item whose cumulative sum exceeds u · total.  If none does
 // (total zero or not finite: data impossible under the model; or rounding at the top end) the last item of positive weight
 // is taken, and item 0 when there is none.
+//
+// Markov jumps (b200SampleMarkovJumps, DESIGN.md §7.2): the same kernels, instantiated with Jumps = true, draw exactly the
+// same sample and look up, per drawn branch pair (i -> j), the conditional expectation N_g,c,r[i][j] of every register g
+// that k_jump_conditional wrote beforehand.  Pattern totals stay in registers; per-(row, pattern) values go to a
+// [g][row][P] workspace that k_jump_branch_totals reduces in a fixed order.
 #include "walk4.cuh"
+
+#include <algorithm>
 
 namespace b200 {
 
@@ -59,12 +66,18 @@ __device__ __forceinline__ void cell4(const AncestralArgs& a, int4 row, int c, i
     }
 }
 
-template <typename T>
+// Markov jumps: n_g of the branch above row r for the drawn pair (i -> j) in category c, looked up in N [g][row][C][S][S]
+__device__ __forceinline__ const double* jumpCell(const AncestralArgs& a, const MarkovJumpArgs& mj, int r, int c, int i, int j) {
+    return mj.cond + (((size_t)r * a.C + c) * a.S + i) * a.S + j;
+}
+
+template <typename T, bool Jumps>
 __global__ void __launch_bounds__(64)
-k_ancestral4(const AncestralArgs a) {
+k_ancestral4(const AncestralArgs a, const MarkovJumpArgs mj) {
     const int p = blockIdx.x * 64 + threadIdx.x;
     if (p >= a.P) return;
     const int S = a.S;
+    double total_g[Jumps ? kMaxJumpRegisters : 1] = {};  // pattern totals, summed in row order
     // root: (c, i) jointly, two passes over the same products so that the running sum reproduces the total exactly
     const int4 root = __ldg(a.rows);
     double total = 0.0;
@@ -126,7 +139,24 @@ k_ancestral4(const AncestralArgs a) {
             if (j < 0) j = lastPos;
         }
         a.outStates[(size_t)r * a.P + p] = j;
+        if constexpr (Jumps) {
+            const double* n = jumpCell(a, mj, r, cat, i, j);
+            const size_t gStride = (size_t)a.count * a.C * S * S;
+#pragma unroll
+            for (int g = 0; g < kMaxJumpRegisters; ++g) {
+                if (g >= mj.G) break;
+                const double v = __ldg(n + g * gStride);
+                total_g[g] += v;
+                if (mj.perRow != nullptr) mj.perRow[((size_t)g * a.count + r) * a.P + p] = v;
+            }
+        }
         prev = j;
+    }
+    if constexpr (Jumps) {
+        if (mj.pattern != nullptr) {
+#pragma unroll
+            for (int g = 0; g < kMaxJumpRegisters; ++g) if (g < mj.G) mj.pattern[(size_t)g * a.P + p] = total_g[g];
+        }
     }
 }
 
@@ -163,11 +193,14 @@ __device__ __forceinline__ int drawWarp(int n, double u, const F& weight) {
     return found >= 0 ? found : last;
 }
 
+// Markov jumps: lane g < G follows register g
+template <bool Jumps>
 __global__ void __launch_bounds__(128)
-k_ancestral_warp(const AncestralArgs a) {
+k_ancestral_warp(const AncestralArgs a, const MarkovJumpArgs mj) {
     const int p = blockIdx.x * 4 + (threadIdx.x >> 5);
     if (p >= a.P) return;                                   // warp-uniform
     const int lane = threadIdx.x & 31, S = a.S, Sp = a.Sp;
+    double total = 0.0;                                     // Markov jumps: lane g's pattern total, in row order
     const double* part = static_cast<const double*>(a.partials);
     auto L = [&](int4 row, int c, int j) -> double {
         if (row.x >= 0) return part[(size_t)row.x * a.stride + ((size_t)c * a.Ppad + p) * Sp + j];
@@ -193,19 +226,163 @@ k_ancestral_warp(const AncestralArgs a) {
                                    [&](int q) { return m[(size_t)q * Sp] * L(row, cat, q); });
         const int j = tipState < S ? tipState : drawn;
         if (lane == 0) a.outStates[(size_t)r * a.P + p] = j;
+        if constexpr (Jumps) {
+            if (lane < mj.G) {
+                const double v = __ldg(jumpCell(a, mj, r, cat, i, j) + (size_t)lane * a.count * a.C * S * S);
+                total += v;
+                if (mj.perRow != nullptr) mj.perRow[((size_t)lane * a.count + r) * a.P + p] = v;
+            }
+        }
         prev = j;
     }
+    if constexpr (Jumps) {
+        if (mj.pattern != nullptr && lane < mj.G) mj.pattern[(size_t)lane * a.P + p] = total;
+    }
+}
+
+// ---- Markov jumps (b200SampleMarkovJumps, DESIGN.md §7.2) -------------------------------------------------------------------
+// With Q = V diag(λ) V^-1 and a register matrix M_g, the expected register total along a branch of time τ jointly with its
+// end state is E = V (W_g ∘ I(τ)) V^-1, W_g = V^-1 M_g V, I_kl(τ) = τ e^{λ_l τ} φ((λ_k - λ_l) τ), φ(x) = expm1(x)/x;
+// conditioned on the end points N = E / P̂ with P̂ = |V diag(e^{λτ}) V^-1| in the k_transition formula and order.
+constexpr int kJumpPanel = 16;                              // output columns per pass of k_jump_conditional
+
+__host__ __device__ constexpr size_t jumpSmemDoubles(int S) { return (size_t)S * S + S + 2 * (size_t)S * kJumpPanel; }
+
+// W_g = V^-1 M_g V, once per call; grid (S, G): block (i, g) writes row i of W_g
+__global__ void __launch_bounds__(128)
+k_jump_registers(const MarkovJumpArgs m, int S) {
+    extern __shared__ double y[];                           // [S]: row i of V^-1 M_g
+    const int i = blockIdx.x, g = blockIdx.y;
+    const double* V = m.eigen;
+    const double* Vi = m.eigen + (size_t)S * S;
+    const double* M = m.registers + (size_t)g * S * S;
+    for (int l = threadIdx.x; l < S; l += blockDim.x) {
+        double acc = 0.0;
+        for (int q = 0; q < S; ++q) acc += Vi[(size_t)i * S + q] * M[(size_t)q * S + l];
+        y[l] = acc;
+    }
+    __syncthreads();
+    for (int l = threadIdx.x; l < S; l += blockDim.x) {
+        double acc = 0.0;
+        for (int q = 0; q < S; ++q) acc += y[q] * V[(size_t)q * S + l];
+        m.W[((size_t)g * S + i) * S + l] = acc;
+    }
+}
+
+// N of every register for one (row r >= 1, category c): grid (count - 1, C).  Shared memory: I [S][S], e^{λτ} [S], and per
+// panel of kJumpPanel output columns P̂ and T = (W_g ∘ I) V^-1 [S][kJumpPanel]; P̂ is computed once per panel, then every
+// register reuses it.  I_kl is evaluated with the larger of λ_k, λ_l in the exponential (the same value, by the symmetry of
+// I): expm1 then never sees a positive argument and cannot overflow.
+__global__ void __launch_bounds__(256)
+k_jump_conditional(const MarkovJumpArgs m, int S, int C, int count) {
+    extern __shared__ double sm[];
+    double* I = sm;
+    double* e = I + (size_t)S * S;
+    double* Pp = e + S;
+    double* T = Pp + (size_t)S * kJumpPanel;
+    const int r = blockIdx.x + 1, c = blockIdx.y;
+    const double* V = m.eigen;
+    const double* Vi = m.eigen + (size_t)S * S;
+    const double* lam = m.eigen + 2 * (size_t)S * S;
+    const double tau = m.lengths[r] * m.rates[c];            // the product k_transition forms
+    for (int k = threadIdx.x; k < S; k += blockDim.x) e[k] = exp(tau * lam[k]);
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < S * S; idx += blockDim.x) {
+        const int k = idx / S, l = idx - k * S;
+        const double x = -fabs(lam[k] - lam[l]) * tau;
+        const double phi = x == 0.0 ? 1.0 : expm1(x) / x;
+        I[idx] = tau * e[lam[k] >= lam[l] ? k : l] * phi;
+    }
+    const size_t gStride = (size_t)count * C * S * S;
+    double* out = m.cond + ((size_t)r * C + c) * S * S;
+    for (int j0 = 0; j0 < S; j0 += kJumpPanel) {
+        const int nj = min(kJumpPanel, S - j0);
+        for (int idx = threadIdx.x; idx < S * nj; idx += blockDim.x) {
+            const int i = idx / nj, jj = idx - i * nj, j = j0 + jj;
+            double acc = 0.0;
+            for (int k = 0; k < S; ++k) acc += V[(size_t)i * S + k] * (e[k] * Vi[(size_t)k * S + j]);
+            Pp[i * kJumpPanel + jj] = fabs(acc);
+        }
+        for (int g = 0; g < m.G; ++g) {
+            const double* W = m.W + (size_t)g * S * S;
+            __syncthreads();                                // I, P̂ written; the previous register's T consumed
+            for (int idx = threadIdx.x; idx < S * nj; idx += blockDim.x) {
+                const int k = idx / nj, jj = idx - k * nj;
+                double acc = 0.0;
+                for (int l = 0; l < S; ++l) acc += (W[(size_t)k * S + l] * I[(size_t)k * S + l]) * Vi[(size_t)l * S + j0 + jj];
+                T[k * kJumpPanel + jj] = acc;
+            }
+            __syncthreads();
+            for (int idx = threadIdx.x; idx < S * nj; idx += blockDim.x) {
+                const int i = idx / nj, jj = idx - i * nj;
+                double E = 0.0;
+                for (int k = 0; k < S; ++k) E += V[(size_t)i * S + k] * T[k * kJumpPanel + jj];
+                const double ph = Pp[i * kJumpPanel + jj];
+                out[(size_t)g * gStride + (size_t)i * S + j0 + jj] = ph > 0.0 ? E / ph : 0.0;
+            }
+        }
+        __syncthreads();                                    // P̂ of this panel consumed
+    }
+}
+
+// branch totals Σ_p w_p n_g[r][p]: grid (count, G), a fixed-order block reduction (no atomics; row 0 is 0)
+__global__ void __launch_bounds__(256)
+k_jump_branch_totals(const MarkovJumpArgs m, int count, int P) {
+    __shared__ double red[256];
+    const int r = blockIdx.x, g = blockIdx.y;
+    double s = 0.0;
+    if (r > 0) {
+        const double* v = m.perRow + ((size_t)g * count + r) * P;
+        for (int p = threadIdx.x; p < P; p += 256) s += m.patternWeights[p] * v[p];
+    }
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) m.branch[(size_t)g * count + r] = red[0];
 }
 
 }  // namespace
 
+bool markovJumpsFit(const Instance* in) {
+    return jumpSmemDoubles(in->S) * sizeof(double) <= std::max<size_t>(in->maxSmemOptin, 48 << 10);
+}
+
+cudaError_t launchMarkovJumps(Instance* in, const AncestralArgs& a, const MarkovJumpArgs& m) {
+    const int S = in->S, C = in->C;
+    k_jump_registers<<<dim3(S, m.G), S <= 32 ? 32 : 128, sizeof(double) * S, in->stream>>>(m, S);
+    if (a.count > 1) {
+        const size_t smem = jumpSmemDoubles(S) * sizeof(double);
+        if (smem > (48 << 10)) {
+            // the device's whole opt-in, never a smaller value: instances on other host threads launch the same kernel
+            const cudaError_t e = cudaFuncSetAttribute(k_jump_conditional, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)in->maxSmemOptin);
+            if (e != cudaSuccess) return e;
+        }
+        const int work = S * std::min(S, kJumpPanel);
+        const int threads = std::min(256, std::max(32, (work + 31) / 32 * 32));
+        k_jump_conditional<<<dim3(a.count - 1, C), threads, smem, in->stream>>>(m, S, C, a.count);
+    }
+    const int blocks4 = (a.P + 63) / 64;
+    if (in->matCP > 0) {
+        if (in->single) k_ancestral4<float, true><<<blocks4, 64, 0, in->stream>>>(a, m);
+        else k_ancestral4<double, true><<<blocks4, 64, 0, in->stream>>>(a, m);
+    } else {
+        k_ancestral_warp<true><<<(a.P + 3) / 4, 128, 0, in->stream>>>(a, m);
+    }
+    if (m.branch != nullptr) k_jump_branch_totals<<<dim3(a.count, m.G), 256, 0, in->stream>>>(m, a.count, a.P);
+    return cudaGetLastError();
+}
+
 cudaError_t launchAncestral(Instance* in, const AncestralArgs& args) {
     if (in->matCP > 0) {
         const int blocks = (args.P + 63) / 64;
-        if (in->single) k_ancestral4<float><<<blocks, 64, 0, in->stream>>>(args);
-        else k_ancestral4<double><<<blocks, 64, 0, in->stream>>>(args);
+        if (in->single) k_ancestral4<float, false><<<blocks, 64, 0, in->stream>>>(args, MarkovJumpArgs{});
+        else k_ancestral4<double, false><<<blocks, 64, 0, in->stream>>>(args, MarkovJumpArgs{});
     } else {
-        k_ancestral_warp<<<(args.P + 3) / 4, 128, 0, in->stream>>>(args);
+        k_ancestral_warp<false><<<(args.P + 3) / 4, 128, 0, in->stream>>>(args, MarkovJumpArgs{});
     }
     return cudaGetLastError();
 }

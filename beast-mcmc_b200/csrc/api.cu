@@ -1281,6 +1281,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->matEigenGen.assign(std::max(1, in->nMatrices), 0u);
     in->eigenGen.assign(std::max(1, in->nEigen), 0u);
     in->eigenReal.assign(std::max(1, in->nEigen), 0);
+    in->eigenKind.assign(std::max(1, in->nEigen), 0);
     in->hEigen.assign((size_t)std::max(1, in->nEigen) * 36, 0.0);
     in->eigenWalk = envInt("B200_EIGEN_WALK", 1);
     in->tipMode = envInt("B200_TIP_MODE", 3);
@@ -1593,6 +1594,9 @@ int beagleSetEigenDecomposition(int instance, int eigenIndex, const double* inEi
     memcpy(pack.data(), inEigenVectors, sizeof(double) * S * S);
     memcpy(pack.data() + S * S, inInverseEigenVectors, sizeof(double) * S * S);
     memcpy(pack.data() + 2 * S * S, inEigenValues, sizeof(double) * (in->complexEigen ? 2 * S : S));
+    bool realSystem = true;
+    if (in->complexEigen) for (size_t k = 0; k < S; ++k) realSystem = realSystem && inEigenValues[S + k] == 0.0;
+    in->eigenKind[eigenIndex] = realSystem ? 1 : 2;
     if (in->matCP > 0) {
         // host copy for the eigen-form walk (V, V^-1 travel by value in its launch); the generation only moves when the
         // content does, so that re-uploading an unchanged system keeps captured graphs valid
@@ -2466,16 +2470,27 @@ int b200SampleAncestralStates(int instance, const int* nodeBuffers, const int* p
                                  stateFrequenciesIndex, seed, drawIndex, 0, outStates, outCategories);
 }
 
+int b200SampleMarkovJumps(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                          const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                          int stateFrequenciesIndex, int eigenIndex, int categoryRatesIndex, const double* registerMatrices,
+                          int registerCount, unsigned long long seed, unsigned long long drawIndex, int* outStates,
+                          int* outCategories, double* outBranchCounts, double* outPatternCounts) {
+    SH(instance, shSampleMarkovJumps(sh, nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer,
+                                     categoryWeightsIndex, stateFrequenciesIndex, eigenIndex, categoryRatesIndex,
+                                     registerMatrices, registerCount, seed, drawIndex, outStates, outCategories,
+                                     outBranchCounts, outPatternCounts));
+    return sampleMarkovJumps(instance, nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer,
+                             categoryWeightsIndex, stateFrequenciesIndex, eigenIndex, categoryRatesIndex, registerMatrices,
+                             registerCount, seed, drawIndex, 0, outStates, outCategories, outBranchCounts, outPatternCounts);
+}
+
 }  // extern "C"
 
-int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
-                                int count, int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex,
-                                unsigned long long seed, unsigned long long drawIndex, int patternOffset, int* outStates,
-                                int* outCategories) {
-    GET_INSTANCE_LAZY(in, instance);
-    // everything is checked before anything is launched, the deferred work of earlier calls included
-    if (outStates == nullptr || outCategories == nullptr ||
-        b200DebugAncestralRows(nodeBuffers, parentRows, matrixIndices, count, in->nBuffers, in->nMatrices) != BEAGLE_SUCCESS ||
+// the sampler's argument rules and the written state of every buffer it reads: checked before anything is launched, the
+// deferred work of earlier calls included
+static int checkSampleRows(Instance* in, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                           int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex) {
+    if (b200DebugAncestralRows(nodeBuffers, parentRows, matrixIndices, count, in->nBuffers, in->nMatrices) != BEAGLE_SUCCESS ||
         !validRange(rootBuffer, in->nBuffers) || !validRange(categoryWeightsIndex, in->nSets) ||
         !validRange(stateFrequenciesIndex, in->nSets))
         return BEAGLE_ERROR_OUT_OF_RANGE;
@@ -2483,6 +2498,15 @@ int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int*
     auto holdsData = [&](int b) { return in->partials[b] != nullptr || in->states32[b] != nullptr; };
     if (!holdsData(rootBuffer)) return BEAGLE_ERROR_OUT_OF_RANGE;
     for (int r = 1; r < count; ++r) if (!holdsData(nodeBuffers[r])) return BEAGLE_ERROR_OUT_OF_RANGE;
+    return BEAGLE_SUCCESS;
+}
+
+// after checkSampleRows: flushes the deferred work, stores virtual cherries, grows the scratch to the sampler's int outputs
+// [categories P | states count x P] followed by `extraDoubles` (*extra), stages the rows and fills the sampler's arguments
+static int prepareSample(Instance* in, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
+                         int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex, unsigned long long seed,
+                         unsigned long long drawIndex, int patternOffset, size_t extraDoubles, AncestralArgs& a,
+                         double** extra) {
     if (!in->pendingMats.empty() || !in->pendingOps.empty()) { const int rc = flushPending(in); if (rc != BEAGLE_SUCCESS) return rc; }
     std::vector<int> bufs(nodeBuffers, nodeBuffers + count);
     bufs[0] = rootBuffer;
@@ -2493,11 +2517,10 @@ int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int*
         rows[r] = make_int4(in->states32[b] != nullptr ? -(b + 1) : in->slotOf[b], r == 0 ? -1 : parentRows[r],
                             r == 0 ? 0 : matrixIndices[r], 0);
     }
-    const size_t outInts = (size_t)(count + 1) * in->P;          // [categories P | states count x P]: ONE D2H copy
-    CUDA_OK(ensureScratch(in, (outInts + 1) / 2));
+    const size_t intDoubles = ((size_t)(count + 1) * in->P + 1) / 2;
+    CUDA_OK(ensureScratch(in, intDoubles + extraDoubles));
     const int4* dRows = static_cast<const int4*>(stage(in, rows.data(), sizeof(int4) * count));
     if (dRows == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
-    AncestralArgs a;
     a.rows = dRows; a.count = count; a.P = in->P; a.Ppad = in->Ppad; a.S = in->S; a.Sp = in->Sp; a.C = in->C; a.CP = in->matCP;
     a.pOffset = patternOffset;
     a.partials = in->partialsBase; a.stride = in->partialsElems;
@@ -2509,12 +2532,88 @@ int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int*
     int* dOut = reinterpret_cast<int*>(in->dScratch);
     a.outCategories = dOut;
     a.outStates = dOut + in->P;
+    if (extra != nullptr) *extra = in->dScratch + intDoubles;
+    return BEAGLE_SUCCESS;
+}
+
+int b200::sampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                int count, int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex,
+                                unsigned long long seed, unsigned long long drawIndex, int patternOffset, int* outStates,
+                                int* outCategories) {
+    GET_INSTANCE_LAZY(in, instance);
+    if (outStates == nullptr || outCategories == nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
+    int rc = checkSampleRows(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex,
+                             stateFrequenciesIndex);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    AncestralArgs a;
+    rc = prepareSample(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex, stateFrequenciesIndex,
+                       seed, drawIndex, patternOffset, 0, a, nullptr);
+    if (rc != BEAGLE_SUCCESS) return rc;
     CUDA_OK(launchAncestral(in, a));
+    const size_t outInts = (size_t)(count + 1) * in->P;          // [categories P | states count x P]: ONE D2H copy
     std::vector<int> host(outInts);
-    CUDA_OK(cudaMemcpyAsync(host.data(), dOut, sizeof(int) * outInts, cudaMemcpyDeviceToHost, in->stream));
+    CUDA_OK(cudaMemcpyAsync(host.data(), a.outCategories, sizeof(int) * outInts, cudaMemcpyDeviceToHost, in->stream));
     CUDA_OK(cudaStreamSynchronize(in->stream));
     memcpy(outCategories, host.data(), sizeof(int) * in->P);
     memcpy(outStates, host.data() + in->P, sizeof(int) * (size_t)count * in->P);
+    return BEAGLE_SUCCESS;
+}
+
+int b200::sampleMarkovJumps(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                            const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                            int stateFrequenciesIndex, int eigenIndex, int categoryRatesIndex, const double* registerMatrices,
+                            int registerCount, unsigned long long seed, unsigned long long drawIndex, int patternOffset,
+                            int* outStates, int* outCategories, double* outBranchCounts, double* outPatternCounts) {
+    GET_INSTANCE_LAZY(in, instance);
+    int rc = checkSampleRows(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex,
+                             stateFrequenciesIndex);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    if (!validRange(eigenIndex, in->nEigen) || in->eigenKind[eigenIndex] == 0 || !validRange(categoryRatesIndex, in->nSets) ||
+        edgeLengths == nullptr || registerMatrices == nullptr || registerCount < 1 || registerCount > kMaxJumpRegisters ||
+        (outBranchCounts == nullptr && outPatternCounts == nullptr))
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    for (int r = 1; r < count; ++r)
+        if (!(std::isfinite(edgeLengths[r]) && edgeLengths[r] >= 0.0)) return BEAGLE_ERROR_OUT_OF_RANGE;
+    if (in->eigenKind[eigenIndex] != 1 || !markovJumpsFit(in)) return BEAGLE_ERROR_NO_IMPLEMENTATION;
+    // scratch after the sampler's ints: M | W [G][S][S], N [G][count][C][S][S], pattern [G][P], branch [G][count] and, for
+    // the branch totals only, the per-(row, pattern) workspace [G][count][P]
+    const size_t G = registerCount, SS = (size_t)in->S * in->S, R = count, P = in->P;
+    const size_t nCond = G * R * in->C * SS, nPerRow = outBranchCounts != nullptr ? G * R * P : 0;
+    AncestralArgs a;
+    double* x = nullptr;
+    rc = prepareSample(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex, stateFrequenciesIndex,
+                       seed, drawIndex, patternOffset, 2 * G * SS + nCond + G * P + G * R + nPerRow, a, &x);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    MarkovJumpArgs m;
+    m.G = registerCount;
+    m.eigen = in->dEigen + (size_t)eigenIndex * (2 * SS + 2 * in->S);
+    m.rates = in->dRates + (size_t)categoryRatesIndex * in->C;
+    double* dM = x;
+    m.registers = dM;
+    m.W = dM + G * SS;
+    m.cond = m.W + G * SS;
+    m.pattern = m.cond + nCond;
+    m.branch = m.pattern + G * P;
+    m.perRow = outBranchCounts != nullptr ? m.branch + G * R : nullptr;
+    if (outBranchCounts == nullptr) m.branch = nullptr;
+    m.patternWeights = in->dPatternWeights;
+    rc = uploadSmall(in, dM, registerMatrices, sizeof(double) * G * SS);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    m.lengths = static_cast<const double*>(stage(in, edgeLengths, sizeof(double) * R));
+    if (m.lengths == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
+    if (outPatternCounts == nullptr) m.pattern = nullptr;
+    CUDA_OK(launchMarkovJumps(in, a, m));
+    // only what was asked for comes back
+    std::vector<int> ints(outStates != nullptr ? (size_t)(count + 1) * P : outCategories != nullptr ? P : 0);
+    if (!ints.empty())
+        CUDA_OK(cudaMemcpyAsync(ints.data(), a.outCategories, sizeof(int) * ints.size(), cudaMemcpyDeviceToHost, in->stream));
+    if (outBranchCounts != nullptr)
+        CUDA_OK(cudaMemcpyAsync(outBranchCounts, m.branch, sizeof(double) * G * R, cudaMemcpyDeviceToHost, in->stream));
+    if (outPatternCounts != nullptr)
+        CUDA_OK(cudaMemcpyAsync(outPatternCounts, m.pattern, sizeof(double) * G * P, cudaMemcpyDeviceToHost, in->stream));
+    CUDA_OK(cudaStreamSynchronize(in->stream));
+    if (outCategories != nullptr) memcpy(outCategories, ints.data(), sizeof(int) * P);
+    if (outStates != nullptr) memcpy(outStates, ints.data() + P, sizeof(int) * R * P);
     return BEAGLE_SUCCESS;
 }
 

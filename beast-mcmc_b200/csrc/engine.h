@@ -177,6 +177,7 @@ struct Instance {
     std::vector<int> matEigen;
     std::vector<unsigned> matEigenGen, eigenGen;
     std::vector<char> eigenReal;
+    std::vector<char> eigenKind;              // any S: 0 = slot never set, 1 = real, 2 = holds complex pairs
     std::vector<double> hEigen;               // [nEigen][32]: V | V^-1 padded to 4 x 4 (host copy, by value into the launch)
     int eigenWalk = 1;                        // B200_EIGEN_WALK: 0 = always the matrix-form kernel
     int tipMode = 2;                          // B200_TIP_MODE: compact tips by contraction (0), P column from global (1), shared-memory column table (2)
@@ -340,5 +341,30 @@ cudaError_t launchAncestral(Instance* in, const AncestralArgs& args);
 int sampleAncestralStates(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
                           int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex, unsigned long long seed,
                           unsigned long long drawIndex, int patternOffset, int* outStates, int* outCategories);
+
+// ---- Markov-jump counts and rewards conditioned on the sampled states (ancestral.cu, DESIGN.md §7.2) ---------------------
+constexpr int kMaxJumpRegisters = 8;
+struct MarkovJumpArgs {
+    int G;                        // registers
+    const double* eigen;          // the eigen slot: V [S][S] | V^-1 [S][S] | eigenvalues (real parts first)
+    const double* rates;          // [C] of the chosen rate set
+    const double* lengths;        // [count] edge lengths (row 0 not read)
+    const double* registers;      // M [G][S][S]
+    double* W;                    // [G][S][S] scratch: V^-1 M_g V
+    double* cond;                 // [G][count][C][S][S] conditional matrices N (row 0 unused)
+    double* perRow;               // [G][count][P] n of every (row, pattern) for the branch totals, or nullptr
+    double* branch;               // [G][count] or nullptr
+    double* pattern;              // [G][P] or nullptr
+    const double* patternWeights; // [Ppad]
+};
+// false when one (row, category) block of the conditional-matrix kernel does not fit in shared memory (S above 154 on an H100)
+bool markovJumpsFit(const Instance* in);
+cudaError_t launchMarkovJumps(Instance* in, const AncestralArgs& a, const MarkovJumpArgs& m);
+// api.cu: b200SampleMarkovJumps on one single-device instance; patternOffset as for sampleAncestralStates
+int sampleMarkovJumps(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                      const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex,
+                      int eigenIndex, int categoryRatesIndex, const double* registerMatrices, int registerCount,
+                      unsigned long long seed, unsigned long long drawIndex, int patternOffset, int* outStates,
+                      int* outCategories, double* outBranchCounts, double* outPatternCounts);
 
 }  // namespace b200

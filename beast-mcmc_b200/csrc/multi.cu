@@ -401,6 +401,44 @@ int shSampleAncestralStates(Sharded* sh, const int* nodeBuffers, const int* pare
     return BEAGLE_SUCCESS;
 }
 
+// as shSampleAncestralStates; the shards' branch totals are added on the host in shard order
+int shSampleMarkovJumps(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                        const double* edgeLengths, int count, int rootBuffer, int wIdx, int fIdx, int eigenIndex, int rIdx,
+                        const double* registerMatrices, int registerCount, unsigned long long seed, unsigned long long drawIndex,
+                        int* outStates, int* outCategories, double* outBranchCounts, double* outPatternCounts) {
+    if (count < 1 || registerCount < 1 || registerCount > kMaxJumpRegisters) return BEAGLE_ERROR_OUT_OF_RANGE;
+    const size_t G = registerCount;
+    std::vector<std::vector<int>> states(sh->g), cats(sh->g);
+    std::vector<std::vector<double>> branch(sh->g), pattern(sh->g);
+    const int rc = sh->pool->run([&](int k) {
+        const size_t n = sh->count[k];
+        if (n == 0) return 0;
+        if (outStates != nullptr) states[k].resize((size_t)count * n);
+        if (outCategories != nullptr) cats[k].resize(n);
+        if (outBranchCounts != nullptr) branch[k].resize(G * count);
+        if (outPatternCounts != nullptr) pattern[k].resize(G * n);
+        auto ptr = [](auto& v) { return v.empty() ? nullptr : v.data(); };
+        return sampleMarkovJumps(sh->child[k], nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer, wIdx,
+                                 fIdx, eigenIndex, rIdx, registerMatrices, registerCount, seed, drawIndex, sh->begin[k],
+                                 ptr(states[k]), ptr(cats[k]), ptr(branch[k]), ptr(pattern[k]));
+    });
+    if (rc != 0) return rc;
+    if (outBranchCounts != nullptr) std::fill(outBranchCounts, outBranchCounts + G * count, 0.0);
+    for (int k = 0; k < sh->g; ++k) {
+        const size_t n = sh->count[k];
+        if (n == 0) continue;
+        if (outCategories != nullptr) memcpy(outCategories + sh->begin[k], cats[k].data(), sizeof(int) * n);
+        if (outStates != nullptr)
+            for (int r = 0; r < count; ++r)
+                memcpy(outStates + (size_t)r * sh->P + sh->begin[k], states[k].data() + (size_t)r * n, sizeof(int) * n);
+        if (outBranchCounts != nullptr) for (size_t q = 0; q < G * count; ++q) outBranchCounts[q] += branch[k][q];
+        if (outPatternCounts != nullptr)
+            for (size_t g = 0; g < G; ++g)
+                memcpy(outPatternCounts + g * sh->P + sh->begin[k], pattern[k].data() + g * n, sizeof(double) * n);
+    }
+    return BEAGLE_SUCCESS;
+}
+
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq) {
     if (outSumSq != nullptr) return BEAGLE_ERROR_NO_IMPLEMENTATION;

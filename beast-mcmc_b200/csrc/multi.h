@@ -17,6 +17,10 @@ int shEdgeDerivatives(Sharded* sh, const int* post, const int* pre, const int* d
 int shSampleAncestralStates(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
                             int rootBuffer, int wIdx, int fIdx, unsigned long long seed, unsigned long long drawIndex,
                             int* outStates, int* outCategories);
+int shSampleMarkovJumps(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                        const double* edgeLengths, int count, int rootBuffer, int wIdx, int fIdx, int eigenIndex, int rIdx,
+                        const double* registerMatrices, int registerCount, unsigned long long seed, unsigned long long drawIndex,
+                        int* outStates, int* outCategories, double* outBranchCounts, double* outPatternCounts);
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq);
 }  // namespace b200

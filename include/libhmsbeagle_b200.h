@@ -393,6 +393,39 @@ BEAGLE_DLLEXPORT int b200SampleAncestralStates(int instance, const int* nodeBuff
                                                const int* matrixIndices, int count, int rootBuffer, int categoryWeightsIndex,
                                                int stateFrequenciesIndex, unsigned long long seed,
                                                unsigned long long drawIndex, int* outStates, int* outCategories);
+/* Markov-jump counts and rewards on the device, conditioned on ONE joint ancestral draw (what
+ * MarkovJumpsBeagleTreeLikelihood computes in Java after each AncestralStateBeagleTreeLikelihood draw; Minin & Suchard 2008,
+ * BEAST's MarkovJumpsCore; DESIGN.md section 7.2).
+ * Rows, seed and drawIndex exactly as in b200SampleAncestralStates: the states and categories drawn are bit-identical to what
+ * b200SampleAncestralStates returns for the same arguments (same Philox counters).
+ *   registerMatrices [registerCount][S][S] row-major, the register-weighted rate matrices M_g the caller forms: counts
+ *          M_ij = Q_ij * R_ij (i != j) with a zero diagonal, rewards M = diag(r).  The engine only sees M.
+ *   eigen system: the real system in slot eigenIndex, Q = V diag(lambda) V^-1.
+ *   time along the branch above row r >= 1: tau = r_c * edgeLengths[r], r_c the rate of the pattern's drawn category c in
+ *          set categoryRatesIndex (edgeLengths[0] is not read).
+ * For every row r >= 1, category c and register g:
+ *   I_kl(tau) = tau * exp(lambda_l tau) * phi((lambda_k - lambda_l) tau), phi(x) = expm1(x) / x, phi(0) = 1
+ *          (evaluated with the larger of lambda_k, lambda_l in the exponential: the same value, no overflow)
+ *   W_g = V^-1 M_g V;  E = V (W_g o I(tau)) V^-1 (o: entrywise);  Phat = |V diag(exp(lambda tau)) V^-1| entrywise, in the
+ *          formula and summation order of the transition matrices;  N[i][j] = E[i][j] / Phat[i][j], 0 where Phat[i][j] = 0
+ *   n_g[r][p] = N_g,c,r[x_parent(r)][x_r] with c and x the drawn category and states (a compact tip's observed state is its
+ *          x); row 0 contributes nothing.
+ * outBranchCounts[g * count + r] = sum_p w_p n_g[r][p] (w the instance's pattern weights: the sum over sites; row 0 is 0),
+ * outPatternCounts[g * patternCount + p] = sum_{r >= 1} n_g[r][p].  outStates [count][patternCount] and outCategories
+ * [patternCount] as in b200SampleAncestralStates; any output may be NULL except both count outputs, and only the outputs
+ * asked for are copied back.  No atomics: repeated calls are bit-identical, the branch totals are summed in a fixed order.
+ * Every error returns before anything is launched (deferred work included) and leaves every output untouched:
+ * BEAGLE_ERROR_OUT_OF_RANGE for whatever b200SampleAncestralStates rejects (its NULL-output rule aside), eigenIndex out of
+ * range or never set, categoryRatesIndex out of range, edgeLengths == NULL or an edgeLengths[r] (r >= 1) negative or not
+ * finite, registerMatrices == NULL, registerCount outside 1..8, both count outputs NULL; BEAGLE_ERROR_NO_IMPLEMENTATION
+ * when the eigen slot holds complex pairs, or when S is so large that one (row, category) block of the conditional matrices
+ * does not fit in the device's shared memory (S above 154 on an H100). */
+BEAGLE_DLLEXPORT int b200SampleMarkovJumps(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                           const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                                           int stateFrequenciesIndex, int eigenIndex, int categoryRatesIndex,
+                                           const double* registerMatrices, int registerCount, unsigned long long seed,
+                                           unsigned long long drawIndex, int* outStates, int* outCategories,
+                                           double* outBranchCounts, double* outPatternCounts);
 /* Host-logic test hook (no CUDA): the row rules of b200SampleAncestralStates for an instance with bufferCount buffers and
  * matrixCount matrices; 0 or BEAGLE_ERROR_OUT_OF_RANGE. */
 BEAGLE_DLLEXPORT int b200DebugAncestralRows(const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
