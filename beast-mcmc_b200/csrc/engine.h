@@ -218,6 +218,7 @@ struct Instance {
     // pinned staging ring for the small per-call arrays (ops, indices, branch lengths)
     char* hStage = nullptr;
     char* dStage = nullptr;
+    char* hStageDev = nullptr;                // hStage as the device addresses it (mapped pinned memory)
     size_t stageSize = 0, stagePos = 0;
     double* hOut = nullptr;                   // pinned result landing zone
 

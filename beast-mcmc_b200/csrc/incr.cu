@@ -7,7 +7,7 @@
 // does all of it, everything travelling BY VALUE in the kernel parameters (no staging copies):
 //   0. every block recomputes the pending branches' spectra exp(lambda_k r_c t) and P(t) into shared memory (a few
 //      hundred flops -- cheaper than a grid-wide dependency on a matrix kernel); block 0 also writes them to HBM in all
-//      the layouts later launches read (exactly what k_transition writes);
+//      the layouts later launches read (exactly what k_transition4 writes);
 //   1. the op list in eigen form, one (pattern, category) cell per thread, the previous op's result forwarded in registers;
 //   2. the root integration on the last op's result while it is still in registers: categories meet through warp shuffles,
 //      site log-likelihoods are stored, the weighted sum is reduced across blocks (fixed order) and the finishing block
@@ -79,7 +79,7 @@ __device__ __forceinline__ void incrementalBody(const IncArgs& A) {
             acc = fabs(acc);
         }
         sP[q][c][j * 4 + i] = acc;
-        if (blockIdx.x == 0) {             // the HBM copies every later launch reads (same layouts as k_transition)
+        if (blockIdx.x == 0) {             // the HBM copies every later launch reads (same layouts as k_transition4)
             double* base = A.mats + (size_t)A.mat[q].prob * A.matStride;
             base[((size_t)j * CP + c) * 4 + i] = acc;
             double* mm = base + 16 * CP;

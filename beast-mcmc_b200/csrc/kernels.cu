@@ -1,6 +1,7 @@
 // kernels.cu -- hand-written sm_90a kernels of the tree-likelihood hot path.
 //
-//   k_transition   : P_c(t) = Evec diag(exp(Eval r_c t)) Ievc           (updateTransitionMatrices)
+//   k_transition4  : P_c(t) = Evec diag(exp(Eval r_c t)) Ievc, 4-state layouts (updateTransitionMatrices)
+//   k_transition   : the same for the generic layout when k_transition_mma does not apply
 //   k_walk4        : 4-state (nucleotide) partials, WARP-OWNED PATTERN COLUMNS walking the whole
 //                    operation list on-device; per-thread shared-memory operand stack (updatePartials)
 //   k_walk_generic : any state count, BLOCK-OWNED pattern tiles walking the list  (updatePartials)
@@ -32,13 +33,14 @@ __device__ __forceinline__ void dmma884acc(double& d0, double& d1, double a, dou
 // ---------------------------------------------------------------------------------------------
 // transition matrices
 // ---------------------------------------------------------------------------------------------
-// grid (count, C); dynamic smem: ec[S], ss[S], pt[S](int).  Follows BaseSubstitutionModel.java:206-241
-// (real) / ComplexColtEigenSystem.java:71-139 (2x2 blocks), abs() convention; output TRANSPOSED.
+// generic layout (matCP == 0).  grid (count, C); dynamic smem: ec[S], ss[S], pt[S](int).  Follows
+// BaseSubstitutionModel.java:206-241 (real) / ComplexColtEigenSystem.java:71-139 (2x2 blocks), abs() convention; output
+// TRANSPOSED.
 __global__ void k_transition(const double* __restrict__ eigenBase, size_t eigenStride, int S, int Sp, int C,
                              int complexForm, const double* __restrict__ ratesBase,
                              const int* __restrict__ probIdx, const int* __restrict__ eigenIdx,
                              const int* __restrict__ rateSet, const double* __restrict__ lengths,
-                             double* __restrict__ matBase, size_t matStride, int matCP, double* __restrict__ evecBase) {
+                             double* __restrict__ matBase, size_t matStride) {
     extern __shared__ double sm[];
     double* ec = sm;
     double* ss = sm + S;
@@ -68,12 +70,8 @@ __global__ void k_transition(const double* __restrict__ eigenBase, size_t eigenS
         }
     }
     __syncthreads();
-    // the branch's spectrum exp(lambda_k r_c t) for the eigen-form walk (walk4e.cu): [matrix][CP][4]
-    if (evecBase != nullptr && threadIdx.x < 4)
-        evecBase[((size_t)probIdx[b] * matCP + c) * 4 + threadIdx.x] = threadIdx.x < S ? ec[threadIdx.x] : 0.0;
-    // generic layout [c][j][i]; 4-state layout [j][CP][i] (one 128-byte line holds row j of all categories)
-    double* out = matBase + (size_t)probIdx[b] * matStride + (matCP ? (size_t)c * 4 : (size_t)c * Sp * Sp);
-    const int rowStride = matCP ? matCP * 4 : Sp;
+    // [c][j][i]
+    double* out = matBase + (size_t)probIdx[b] * matStride + (size_t)c * Sp * Sp;
     for (int idx = threadIdx.x; idx < Sp * Sp; idx += blockDim.x) {
         int j = idx / Sp, i = idx % Sp;          // out[j][i] = P[i][j]
         double acc = 0.0;
@@ -84,25 +82,126 @@ __global__ void k_transition(const double* __restrict__ eigenBase, size_t eigenS
             }
             acc = fabs(acc);
         }
-        out[(size_t)j * rowStride + i] = acc;
-        if (!matCP) {
-            // generic layout: second half of the buffer holds the row-major M[c][i][j] (tensor-path B operand)
-            const size_t ld = (size_t)Sp + 4;
-            double* padded = matBase + (size_t)probIdx[b] * matStride + (size_t)C * Sp * Sp;
-            padded[((size_t)c * Sp + i) * ld + j] = acc;                                   // M[c][i][.]
-            padded[(size_t)C * Sp * ld + ((size_t)c * Sp + j) * ld + i] = acc;             // MT[c][j][.]
+        out[(size_t)j * Sp + i] = acc;
+        // second half of the buffer holds the row-major M[c][i][j] (tensor-path B operand)
+        const size_t ld = (size_t)Sp + 4;
+        double* padded = matBase + (size_t)probIdx[b] * matStride + (size_t)C * Sp * Sp;
+        padded[((size_t)c * Sp + i) * ld + j] = acc;                                   // M[c][i][.]
+        padded[(size_t)C * Sp * ld + ((size_t)c * Sp + j) * ld + i] = acc;             // MT[c][j][.]
+    }
+}
+
+// 4-state layout (matCP > 0, Sp == 4).  One quad of lanes per (branch, category), kTransition4Block-thread blocks over
+// count x C quads.  The branch records (length and the matrix, eigen and rate-set indices) are read where the host staged
+// them, in pinned memory over PCIe: the first threads of a block fetch the block's few contiguous records into shared
+// memory once, so that every record crosses the bus in a handful of wide requests instead of once per warp that uses it.
+// Lane k of a quad forms exp(d lambda_k) -- and for a complex pair the cos/sin terms and the partner row pt -- with
+// k_transition's expressions and hands them to the other three lanes by shuffle.  Lane k = 2g + h then forms the 2 x 2 tile
+// P[2h..2h+1][2g..2g+1]: that way each 16-byte store of the quad fills whole 32-byte sectors in every copy below (row-major
+// P and its transpose alike), where a lane holding a whole row would write each sector in two halves.  Every product and
+// sum is an explicit _rn operation in the order k_transition compiles to (iexp = fma(ec_m, Ievc[m][j], ss_m * Ievc[pt_m][j]),
+// acc = fma(Evec[i][m], iexp, acc) from +0, m ascending), so both give the same bits and ptxas cannot contract otherwise.
+// Writes, per (branch, category):
+//   [j][CP][i]    : row j of all categories is one 128-byte line (k_walk4*, k_walk4e matrix form, getTransitionMatrix)
+//   [matrix][CP][4] spectrum exp(lambda_k r_c t) for the eigen-form walk (walk4e.cu)
+//   Mpad[c][8][4] : B fragment of k_walk4t, lane (g,t) reads [g][t]; rows g >= 4 stay zero
+//   MTg [c][5][4] : column s of P for a compact tip in state s, plus the gap column s == S = (1,..,1,0..)
+constexpr int kTransition4Block = 256;
+__global__ void __launch_bounds__(kTransition4Block)
+k_transition4(const double* __restrict__ eigenBase, size_t eigenStride, int S, int C, int CP, int complexForm,
+              const double* __restrict__ ratesBase, const int* __restrict__ probIdx, const int* __restrict__ eigenIdx,
+              const int* __restrict__ rateSet, const double* __restrict__ lengths, int count,
+              double* __restrict__ matBase, size_t matStride, double* __restrict__ evecBase) {
+    constexpr int Q = kTransition4Block / 4;                      // quads per block: at most Q branches (C = 1)
+    __shared__ double sLen[Q];
+    __shared__ int sProb[Q], sEig[Q], sRate[Q];
+    const int lane = threadIdx.x & 31, k = lane & 3, i0 = 2 * (k & 1), j0 = 2 * (k >> 1);   // tile rows i0.., columns j0..
+    const unsigned quad = 0xFu << (lane & ~3);
+    const int q = (int)(blockIdx.x * (unsigned)Q + (threadIdx.x >> 2));
+    const int bFirst = (int)(blockIdx.x * (unsigned)Q) / C;
+    const int nb = min(count, ((int)(blockIdx.x * (unsigned)Q) + Q - 1) / C + 1) - bFirst;
+    if ((int)threadIdx.x < nb) {
+        sLen[threadIdx.x] = lengths[bFirst + threadIdx.x];
+        sProb[threadIdx.x] = probIdx[bFirst + threadIdx.x];
+        sEig[threadIdx.x] = eigenIdx[bFirst + threadIdx.x];
+        sRate[threadIdx.x] = rateSet[bFirst + threadIdx.x];
+    }
+    __syncthreads();
+    if (q >= count * C) return;                                   // whole quads leave together
+    const int b = q / C, c = q - b * C, r = b - bFirst;
+    const double* E = eigenBase + (size_t)sEig[r] * eigenStride;
+    const double* evec = E;
+    const double* ievc = E + (size_t)S * S;
+    const double* eval = E + 2 * (size_t)S * S;
+    const double d = __dmul_rn(sLen[r], ratesBase[(size_t)sRate[r] * C + c]);
+    // the tile's rows of Evec and columns of Ievc do not depend on the exponentials: in flight while those are formed
+    double V[2][4], W[4][2];
+#pragma unroll
+    for (int m = 0; m < 4; ++m)
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+            V[t][m] = (i0 + t < S && m < S) ? evec[(size_t)(i0 + t) * S + m] : 0.0;
+            W[m][t] = (m < S && j0 + t < S) ? ievc[(size_t)m * S + j0 + t] : 0.0;
+        }
+    double ec = 0.0, ss = 0.0;
+    int pt = k;
+    if (k < S) {
+        const double im = complexForm ? eval[S + k] : 0.0;
+        if (im == 0.0) {
+            ec = exp(__dmul_rn(d, eval[k]));
         } else {
-            // tensor-path copies after the [j][CP][i] block (k_walk4t):
-            //   Mpad[c][8][4] : B fragment, lane (g,t) reads [g][t]; rows g >= 4 stay zero
-            //   MTg [c][5][4] : column s of P for a compact tip in state s, plus the gap column s == S = (1,..,1,0..)
-            double* mm = matBase + (size_t)probIdx[b] * matStride + 16 * matCP;
-            mm[(size_t)c * 32 + i * 4 + j] = acc;
-            mm[(size_t)c * 32 + 16 + i * 4 + j] = 0.0;
-            double* mt = mm + (size_t)C * 32;
-            mt[(size_t)c * 20 + j * 4 + i] = (j < S) ? acc : ((j == S && i < S) ? 1.0 : 0.0);
-            if (j == 0) mt[(size_t)c * 20 + 16 + i] = (S == 4 && i < S) ? 1.0 : 0.0;
+            // rows of a conjugate pair are adjacent; the FIRST row's imaginary part drives the block
+            int run = 0;
+            for (int m = k - 1; m >= 0 && eval[S + m] != 0.0; --m) ++run;
+            const bool first = (run % 2 == 0);
+            const int k0 = first ? k : k - 1;
+            const double bb = eval[S + k0];
+            const double expat = exp(__dmul_rn(d, eval[k0]));
+            ec = __dmul_rn(expat, cos(__dmul_rn(d, bb)));
+            ss = __dmul_rn(__dmul_rn(first ? 1.0 : -1.0, expat), sin(__dmul_rn(d, bb)));
+            pt = first ? k + 1 : k - 1;
         }
     }
+    double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};                  // acc[a][t] = P[i0 + a][j0 + t] before abs()
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+        const double ecm = __shfl_sync(quad, ec, m, 4);
+        const double ssm = __shfl_sync(quad, ss, m, 4);
+        const int ptm = __shfl_sync(quad, pt, m, 4);
+        if (m < S) {
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+                // the partner row of a complex pair is read where k_transition reads it
+                const double wp = (ptm == m || j0 + t >= S) ? W[m][t] : ievc[(size_t)ptm * S + j0 + t];
+                const double iexp = __fma_rn(ecm, W[m][t], __dmul_rn(ssm, wp));
+#pragma unroll
+                for (int a = 0; a < 2; ++a) acc[a][t] = __fma_rn(V[a][m], iexp, acc[a][t]);
+            }
+        }
+    }
+    double p[2][2], g[2][2];                                      // the tile after abs(); the same as MTg entries [j][i]
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+            const int i = i0 + a, j = j0 + t;
+            p[a][t] = (i < S && j < S) ? fabs(acc[a][t]) : 0.0;
+            g[a][t] = (j < S) ? p[a][t] : ((j == S && i < S) ? 1.0 : 0.0);
+        }
+    const int mat = sProb[r];
+    double* base = matBase + (size_t)mat * matStride;
+    double* mm = base + 16 * (size_t)CP + (size_t)c * 32;
+    double* mt = base + 16 * (size_t)CP + (size_t)C * 32 + (size_t)c * 20;
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+        // row j0 + t of [j][CP][i] and of MTg, entries i0, i0 + 1; row i0 + t of Mpad, entries j0, j0 + 1
+        *reinterpret_cast<double2*>(base + ((size_t)(j0 + t) * CP + c) * 4 + i0) = make_double2(p[0][t], p[1][t]);
+        *reinterpret_cast<double2*>(mt + (j0 + t) * 4 + i0) = make_double2(g[0][t], g[1][t]);
+        *reinterpret_cast<double2*>(mm + (i0 + t) * 4 + j0) = make_double2(p[t][0], p[t][1]);
+        *reinterpret_cast<double2*>(mm + 16 + 8 * t + 2 * k) = make_double2(0.0, 0.0);
+    }
+    mt[16 + k] = S == 4 ? 1.0 : 0.0;
+    evecBase[((size_t)mat * CP + c) * 4 + k] = k < S ? ec : 0.0;
 }
 
 // convolveTransitionMatrices / addTransitionMatrices (SubstitutionModelDelegate.java:303-470, epoch and branch-specific
@@ -227,7 +326,14 @@ static cudaError_t launchTransitionMmaT(Instance* in, const int* dProbIdx, const
 cudaError_t launchTransitionMatrices(Instance* in, const int* dProbIdx, const int* dEigenIdx,
                                      const int* dRateSet, const double* dLengths, int count) {
     if (count <= 0) return cudaSuccess;
-    if (in->genericMma && in->matCP == 0 && !in->complexEigen) {
+    if (in->matCP > 0) {
+        const unsigned blocks = (unsigned)(((size_t)count * in->C * 4 + kTransition4Block - 1) / kTransition4Block);
+        k_transition4<<<blocks, kTransition4Block, 0, in->stream>>>(in->dEigen, 2 * (size_t)in->S * in->S + 2 * in->S, in->S, in->C,
+                                                      in->matCP, in->complexEigen ? 1 : 0, in->dRates, dProbIdx, dEigenIdx,
+                                                      dRateSet, dLengths, count, in->dMat, in->matStride, in->dEvec);
+        return cudaGetLastError();
+    }
+    if (in->genericMma && !in->complexEigen) {
         switch (in->Sp / 8) {
             case 1: return launchTransitionMmaT<1>(in, dProbIdx, dEigenIdx, dRateSet, dLengths, count);
             case 2: return launchTransitionMmaT<2>(in, dProbIdx, dEigenIdx, dRateSet, dLengths, count);
@@ -243,7 +349,7 @@ cudaError_t launchTransitionMatrices(Instance* in, const int* dProbIdx, const in
     k_transition<<<grid, threads, smem, in->stream>>>(in->dEigen, 2 * (size_t)in->S * in->S + 2 * in->S, in->S,
                                                       in->Sp, in->C, in->complexEigen ? 1 : 0, in->dRates,
                                                       dProbIdx, dEigenIdx, dRateSet, dLengths, in->dMat,
-                                                      in->matStride, in->matCP, in->matCP ? in->dEvec : nullptr);
+                                                      in->matStride);
     return cudaGetLastError();
 }
 

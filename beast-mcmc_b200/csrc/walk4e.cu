@@ -7,7 +7,7 @@
 // Here no transition matrix is read at all.  With one real eigen system per list (what HomogenousSubstitutionModelDelegate
 // hands over, HSMD:228-266)
 //        P_c(t) x = V ( e ⊙ (V^-1 x) ),     e_k = exp(lambda_k r_c t)
-// so a branch is 4 doubles per category ("spectrum", written by k_transition next to the matrices) and V, V^-1 are the same
+// so a branch is 4 doubles per category ("spectrum", written by k_transition4 next to the matrices) and V, V^-1 are the same
 // for every op of the launch: they travel BY VALUE in the kernel parameters, i.e. in the constant bank, and reach the FP64
 // pipe as uniform-register operands (SASS: LDCU.128 + DFMA R, R, UR, R) -- zero registers, zero LSU wavefronts.
 //   internal child : u = V^-1 x (16 FMA), w = e ⊙ u (4), y = |V w| (16)        -- 32 B of spectrum instead of 128 B of matrix
