@@ -255,9 +255,9 @@ char gImplDesc[] = "sm_90a walk kernels: one launch per operation list, shared-m
 //     which multiplies the warps in flight (latency hiding) and shortens the dependent chain from
 //     n ops to ~phases*T;
 //   * inside a subtree ops run in Sethi-Ullman order (deeper-need child first), which minimises the
-//     number of live intermediate results = operand-stack slots;
-//   * results crossing a phase boundary go through global memory (L2), everything else through the
-//     shared-memory stack.
+//     number of live intermediate results;
+//   * every result is stored to global memory; inside a subtree walk the next op may take it from registers
+//     (forwardFromPrevious) and a later one from the sibling stack (assignStackSlots).
 // Lists with hazards the forest model does not cover (a buffer written twice, read-before-write,
 // a result consumed by two ops) run as ONE subtree in the caller's order.
 struct Sub { int begin, end, pBase, pLimit; };     // op positions [begin,end) applied to patterns [pBase,pLimit)
@@ -519,8 +519,7 @@ void assignStackSlots(std::vector<Op4>& ops, const std::vector<Sub>& subs, int d
 // nSnap: virtual cherries the list produces (their recipes are snapshot first); virt: the records name virtual cherries;
 // phaseSlots: sibling-stack depth of each phase (eigen-form walks)
 cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const std::vector<int>& phaseStart,
-                       const std::vector<int>& phaseDepth, const std::vector<int>& phaseSlots, bool fourPath, int maxWindow,
-                       bool preOrder, int eigenSlot = -1,
+                       const std::vector<int>& phaseSlots, bool fourPath, int maxWindow, bool preOrder, int eigenSlot = -1,
                        bool aligned = false, const void* dSnap = nullptr, int nSnap = 0, const void* dVirtTips = nullptr) {
     const bool virt = dVirtTips != nullptr;
     cudaError_t e = cudaSuccess;
@@ -532,15 +531,15 @@ cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const 
         const int s0 = phaseStart[ph], s1 = phaseStart[ph + 1];
         if (s1 <= s0) continue;
         TimedScope ts(in, T_PARTIALS);
-        if (fourPath && eigenSlot >= 0 && !preOrder && (ph >= phaseDepth.size() || phaseDepth[ph] == 0)) {
+        if (fourPath && eigenSlot >= 0 && !preOrder) {
             e = launchWalk4E(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
                              aligned, in->hEigen.data() + (size_t)eigenSlot * 36, static_cast<const int4*>(dVirtTips),
                              ph < phaseSlots.size() ? phaseSlots[ph] : 0);
             continue;
         }
         if (virt) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
-        e = fourPath ? launchWalk4(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0,
-                                   ph < phaseDepth.size() ? phaseDepth[ph] : 0, maxWindow, preOrder)
+        e = fourPath ? launchWalk4(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
+                                   preOrder)
                      : launchWalkGeneric(in, static_cast<const DevOp*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0,
                                          maxWindow, preOrder);
     }
@@ -653,7 +652,7 @@ int prepareOps(Instance* in, const std::vector<HostOp>& hops, bool byPartition) 
 // The eigen-form walk serves a post-order 4-state list when every matrix it names was computed by
 // updateTransitionMatrices from the CURRENT content of ONE real eigen slot; returns that slot or -1.
 int eigenFormSlot(const Instance* in, const std::vector<HostOp>& hops) {
-    if (!in->eigenWalk || in->matCP == 0 || in->walkVariant != 0 || hops.empty() || hops[0].kind == 1) return -1;
+    if (!in->eigenWalk || in->matCP == 0 || hops.empty() || hops[0].kind == 1) return -1;
     const int E = in->matEigen[hops[0].m1];
     if (E < 0 || !in->eigenReal[E]) return -1;
     const unsigned gen = in->eigenGen[E];
@@ -709,7 +708,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                 if (cp.graphExec == nullptr && !cp.graphFailed && cp.hits >= 2 && !in->timing &&
                     cudaStreamBeginCapture(in->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
                     const cudaError_t e1 = launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart,
-                                                      cp.phaseDepth, cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
+                                                      cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
                                                       !cp.byPartition, dSnap, nSnap, dTips);
                     cp.graphEigen = eigenSlot;
                     cp.graphEigenGen = eigenGenNow;
@@ -724,7 +723,6 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                         cp.graph = g;
                         cp.graphKernelNodes.clear();
                         cp.graphAllEigen = cp.fourPath && eigenSlot >= 0 && !cp.preOrder;
-                        for (int dpt : cp.phaseDepth) cp.graphAllEigen = cp.graphAllEigen && dpt == 0;
                         size_t nn = 0;
                         if (cudaGraphGetNodes(g, nullptr, &nn) == cudaSuccess && nn > 0) {
                             std::vector<cudaGraphNode_t> nodes(nn);
@@ -749,9 +747,8 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                     return BEAGLE_SUCCESS;
                 }
             }
-            CUDA_OK(launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart, cp.phaseDepth,
-                               cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap,
-                               dTips));
+            CUDA_OK(launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart, cp.phaseSlots,
+                               cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap, dTips));
             CUDA_OK(accumulateInList(in, cp.cumGroups));
             noteScaleWrites(in, hops);
             noteCherryWrites(in, hops, cp.cherries);
@@ -774,7 +771,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     std::vector<int4> snap;
     std::vector<HostOp> kept;
     bool readsVirtual = false;
-    if (!in->cherryTip1.empty() && !byPartition && !preOrder && eigenSlot >= 0 && !in->stackTail) {
+    if (!in->cherryTip1.empty() && !byPartition && !preOrder && eigenSlot >= 0) {
         std::vector<int> writes(in->nBuffers, 0), firstRead(in->nBuffers, n);
         for (int k = 0; k < n; ++k) {
             writes[hops[k].dest]++;
@@ -799,8 +796,8 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     }
     Plan plan;
     int maxWindow = in->Ppad;
-    // patterns one warp owns: FMA kernel (32/CP)*R, tensor kernels 8*R resp. 16
-    const int patsPerWarp = !fourState ? 16 : (in->walkVariant == 2 ? 8 * in->tensorR : (32 / in->matCP) * in->walkR);
+    // patterns one warp owns: 4-state kernels (32/CP)*R, S > 4 tensor kernel 16
+    const int patsPerWarp = !fourState ? 16 : (32 / in->matCP) * in->walkR;
     const int warpsPerSM = fourState ? 32 : 12;      // resident warps the kernel family can hold per SM
     auto wantSubsFor = [&](int window) {
         const int warpsPerSub = std::max(1, (window + patsPerWarp - 1) / patsPerWarp);
@@ -899,56 +896,10 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
     }
     const std::vector<int>& order = plan.order;
 
-    // ---- stack slots (4-state path only): one backward pass finds, for every produced value, the
-    // position of its LAST reader inside this list (before the buffer is re-written); the forward
-    // pass then parks results in slots and frees each slot at that last read.
-    // The operand stack pays off where a phase is LATENCY-bound (few walks in flight: the tail of a full
-    // evaluation, or the short dependent chain of an incremental update): it removes the store -> L2 -> load round
-    // trip from every op of the chain.  Throughput-bound phases run without it (shared memory would cap occupancy).
-    const bool stackEverywhere = fourState && in->walkVariant == 1 && !preOrder;
-    const bool stackThin = fourState && in->walkVariant == 0 && in->stackTail && !preOrder;
-    const int maxDepth = (stackEverywhere || stackThin) ? in->stackDepthMax : 0;
     const int nPhases = (int)plan.phaseStart.size() - 1;
-    std::vector<char> subStack(plan.subs.size(), 0);
-    std::vector<int> phaseDepth(std::max(nPhases, 1), 0), phaseOfSub(plan.subs.size(), 0);
-    if (maxDepth > 0) {
-        const int patsPerWarpS = (32 / in->matCP) * in->walkR;
-        for (int ph = 0; ph < nPhases; ++ph) {
-            long warps = 0;
-            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) {
-                warps += (plan.subs[q].pLimit - plan.subs[q].pBase + patsPerWarpS - 1) / patsPerWarpS;
-                phaseOfSub[q] = ph;
-            }
-            const bool thin = warps < (long)in->smCount * 8;
-            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) subStack[q] = stackEverywhere || thin;
-        }
-    }
-    std::vector<int> lastReadOfProd(maxDepth > 0 ? nL : 0, -1);
     std::vector<int> subOfPos(nL, 0);
     for (int sIdx = 0; sIdx < (int)plan.subs.size(); ++sIdx)
         for (int q = plan.subs[sIdx].begin; q < plan.subs[sIdx].end; ++q) subOfPos[q] = sIdx;
-    if (maxDepth > 0) {
-        // per subtree: the stack is private to a (subtree, tile) walk
-        std::vector<int> lastRead(in->nBuffers, -1);
-        for (size_t sIdx = 0; sIdx < plan.subs.size(); ++sIdx) {
-            if (!subStack[sIdx]) continue;
-            const Sub& sb = plan.subs[sIdx];
-            for (int pos = sb.end - 1; pos >= sb.begin; --pos) {
-                const HostOp& o = L[order[pos]];
-                lastReadOfProd[pos] = lastRead[o.dest];
-                lastRead[o.dest] = -1;
-                if (lastRead[o.c1] < 0) lastRead[o.c1] = pos;
-                if (lastRead[o.c2] < 0) lastRead[o.c2] = pos;
-            }
-            for (int pos = sb.begin; pos < sb.end; ++pos) {      // leave no marks for the next subtree
-                const HostOp& o = L[order[pos]];
-                lastRead[o.dest] = lastRead[o.c1] = lastRead[o.c2] = -1;
-            }
-        }
-    }
-    std::vector<int> slotOf(maxDepth > 0 ? in->nBuffers : 0, -1), slotFreeAt(maxDepth > 0 ? in->nBuffers : 0, -1);
-    std::vector<int> freeSlots;
-    int depthUsed = 0, depthThisSub = 0, curSub = -1;
 
     const bool fourPath = in->matCP > 0;
     std::vector<CumGroup> cumGroups;
@@ -959,33 +910,6 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         const HostOp& o = L[order[pos]];
         const bool t1 = in->states32[o.c1] != nullptr;
         const bool t2 = in->states32[o.c2] != nullptr;
-        int srcSlot1 = -1, srcSlot2 = -1, dstSlot = -1;
-        if (maxDepth > 0 && subOfPos[pos] != curSub) {      // new subtree: fresh private stack
-            curSub = subOfPos[pos];
-            freeSlots.clear();
-            depthThisSub = 0;
-        }
-        if (maxDepth > 0 && subStack[subOfPos[pos]]) {
-            auto take = [&](int buf, bool isTip) -> int {
-                if (isTip) return -1;
-                const int slot = slotOf[buf];
-                if (slot >= 0 && slotFreeAt[buf] == pos) { freeSlots.push_back(slot); slotOf[buf] = -1; }
-                return slot;
-            };
-            srcSlot1 = take(o.c1, t1);
-            srcSlot2 = (o.c2 == o.c1) ? srcSlot1 : take(o.c2, t2);
-            if (slotOf[o.dest] >= 0) { freeSlots.push_back(slotOf[o.dest]); slotOf[o.dest] = -1; }   // stale value
-            if (lastReadOfProd[pos] > pos) {         // a later op of this list reads the result
-                int slot = -1;
-                if (!freeSlots.empty()) { slot = freeSlots.back(); freeSlots.pop_back(); }
-                else if (depthThisSub < maxDepth) {
-                    slot = depthThisSub++;
-                    depthUsed = std::max(depthUsed, depthThisSub);
-                    phaseDepth[phaseOfSub[subOfPos[pos]]] = std::max(phaseDepth[phaseOfSub[subOfPos[pos]]], depthThisSub);
-                }
-                if (slot >= 0) { slotOf[o.dest] = slot; slotFreeAt[o.dest] = lastReadOfProd[pos]; dstSlot = slot; }
-            }
-        }
         const int pBegin = byPartition ? in->partBegin[o.part] : 0;
         const int pEnd = byPartition ? in->partEnd[o.part] : in->P;
         // In-list cumulative scaling (cumulativeScaleIndex != NONE) is NOT done inside the walk: independent subtrees of a
@@ -1007,12 +931,12 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             d.c2 = t2 ? -(o.c2 + 1) : v2 ? o.c2 : in->slotOf[o.c2];
             d.m1 = o.m1; d.m2 = o.m2; d.sw = o.sw; d.sr = o.sr; d.cum = cum;
             d.pBegin = pBegin; d.pEnd = pEnd;
-            d.slots = (unsigned)(srcSlot1 & 0xFF) | ((unsigned)(srcSlot2 & 0xFF) << 8) | ((unsigned)(dstSlot & 0xFF) << 16);
+            d.slots = 0xFFFFFFu;                              // no sibling-stack slots until assignStackSlots
             d.pad_ = o.kind | (v1 ? 4 : 0) | (v2 ? 8 : 0);
             d.pfA = d.pfB = 0; d.pfM1 = d.pfM2 = -1;
             if (readsVirtual)
                 virtTips[pos] = make_int4(v1 ? vt1[o.c1] : 0, v1 ? vt2[o.c1] : 0, v2 ? vt1[o.c2] : 0, v2 ? vt2[o.c2] : 0);
-            if (in->forward && !(maxDepth > 0 && subStack[subOfPos[pos]]) && pos > plan.subs[subOfPos[pos]].begin)
+            if (in->forward && pos > plan.subs[subOfPos[pos]].begin)
                 forwardFromPrevious(d, ops4[pos - 1], preOrder, readsVirtual ? &virtTips[pos] : nullptr);
         } else {
             DevOp& d = dops[pos];
@@ -1028,7 +952,6 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             d.scaleRead = o.sr >= 0 ? in->dScale + (size_t)o.sr * in->Ppad : nullptr;
             d.cumScale = cum >= 0 ? in->dScale + (size_t)cum * in->Ppad : nullptr;
             d.pBegin = pBegin; d.pEnd = pEnd;
-            d.srcSlot1 = d.srcSlot2 = d.dstSlot = -1;
             d.pad_ = o.kind;
             // register forwarding on the tensor-pipe walk (one category): the warp that wrote the previous op's 16-pattern
             // tile still holds it in its accumulators -- flag the child (moved to position 1; the product commutes exactly)
@@ -1043,10 +966,10 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             }
         }
     }
-    // sibling stack: lists whose phases the staged eigen walk may run (post-order, aligned, no matrix-form stack)
+    // sibling stack: lists whose phases the staged eigen walk may run (post-order, aligned)
     std::vector<int> phaseSlots(std::max(nPhases, 1), 0);
     long fromStack = 0, fromMemory = 0;
-    if (fourPath && eigenSlot >= 0 && !preOrder && !byPartition && maxDepth == 0 && in->stackSlots > 0 && walkStackBuilt(in)) {
+    if (fourPath && eigenSlot >= 0 && !preOrder && !byPartition && in->stackSlots > 0 && walkStackBuilt(in)) {
         std::vector<int> subDepth;
         assignStackSlots(ops4, plan.subs, in->stackSlots, subDepth, fromStack, fromMemory);
         for (int ph = 0; ph < nPhases; ++ph)
@@ -1063,7 +986,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) thick[q] = t;
         }
         for (size_t sIdx = 0; sIdx < plan.subs.size(); ++sIdx) {
-            if ((maxDepth > 0 && subStack[sIdx]) || (!thick[sIdx] && in->lookahead < 2)) continue;
+            if (!thick[sIdx] && in->lookahead < 2) continue;
             for (int pos = plan.subs[sIdx].begin; pos + 1 < plan.subs[sIdx].end; ++pos) {
                 Op4& d = ops4[pos];
                 const Op4& nx = ops4[pos + 1];
@@ -1111,9 +1034,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
         if (ce != cudaSuccess) { cudaFree(tmp); CUDA_OK(ce); }
     }
     void* dSubs = static_cast<char*>(dOps) + subsOffset;
-    std::vector<int> depths(plan.phaseStart.size(), 0);
-    for (size_t ph = 0; ph + 1 < plan.phaseStart.size(); ++ph) depths[ph] = (maxDepth > 0 && ph < phaseDepth.size()) ? phaseDepth[ph] : 0;
-    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, depths, phaseSlots, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
+    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, phaseSlots, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
                                static_cast<char*>(dOps) + snapOffset, (int)snap.size(),
                                readsVirtual ? static_cast<char*>(dOps) + tipsOffset : nullptr);
     if (e == cudaSuccess) e = accumulateInList(in, cumGroups);
@@ -1141,8 +1062,7 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
             slot->key = hops; slot->n = n; slot->byPartition = byPartition; slot->epoch = in->bufferEpoch;
             slot->subsOffset = subsOffset; slot->snapOffset = snapOffset; slot->tipsOffset = tipsOffset;
             slot->cherries = cherries; slot->external = external; slot->readsVirtual = readsVirtual;
-            slot->phaseStart = plan.phaseStart; slot->phaseDepth = depths;
-            slot->phaseSlots = phaseSlots;
+            slot->phaseStart = plan.phaseStart; slot->phaseSlots = phaseSlots;
             slot->fourPath = fourPath; slot->maxWindow = maxWindow; slot->preOrder = preOrder;
             slot->lastUse = ++in->planClock;
             slot->cumGroups = cumGroups;
@@ -1271,8 +1191,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
         int cp = 1;
         while (cp < in->C) cp <<= 1;
         in->matCP = cp;
-        in->matStride = (size_t)16 * cp + 52 * (size_t)in->C;     // [j][CP][i] + Mpad[c][8][4] + MTg[c][5][4]
-        in->matStride = (in->matStride + 3) & ~size_t(3);        // keep every buffer 32-byte aligned
+        in->matStride = (size_t)16 * cp;                          // [j][CP][i]: every buffer stays 32-byte aligned
     } else {
         in->matCP = 0;
         // MT[c][j][i] (FMA walk, tip gathers), then the tensor-path operands with an (Sp+4)-double row stride so that ONE
@@ -1295,7 +1214,6 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->thinTipMode = envInt("B200_THIN_TIP_MODE", in->tipMode);
     in->virtualCherries = envInt("B200_VIRTUAL_CHERRIES", 1);
     in->walkBlock = 128;
-    in->walkVariant = envInt("B200_WALK_VARIANT", 0);
     in->reorder = envInt("B200_REORDER", 1);
     in->forward = envInt("B200_FORWARD", 1);
     in->stackSlots = envInt("B200_WALK_STACK_SLOTS", 1) != 0 ? kStackSlots : 0;
@@ -1307,14 +1225,12 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->planCacheSize = std::max(0, std::min(16, envInt("B200_PLAN_CACHE", 4)));
     in->planCache.reserve(16);
     in->thinR1 = envInt("B200_THIN_R1", 1);
-    in->stackTail = envInt("B200_STACK_TAIL", 0);     // measured slower (0.458 vs 0.436 ms): off by default
     in->phaseT = envInt("B200_PHASE_T", 0);
     in->phaseTmin = std::max(1, envInt("B200_PHASE_TMIN", 4));
     in->phaseSmall = envInt("B200_PHASE_SMALL", 24);
     in->phaseOversub = std::max(0, envInt("B200_PHASE_OVERSUB", 0));      // 0 = by subtree width (see wantSubsFor)
     in->walkMinBlocks = envInt("B200_WALK_MINB", 4);
     in->walkMinBlocksSet = getenv("B200_WALK_MINB") != nullptr;
-    in->tensorR = envInt("B200_TENSOR_R", 2) >= 4 ? 4 : 2;
     in->genericMma = envInt("B200_GENERIC_MMA", 1);
     in->mmaWarps = envInt("B200_MMA_WARPS", 4) == 8 ? 8 : 4;     // 8 = 256-thread blocks with cp.async double buffering
     // the SM count sizes the walk below: query the device first
@@ -1329,8 +1245,6 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
         const int G = 32 / in->matCP;
         while (in->walkR > 1 && (in->Ppad + G * in->walkR - 1) / (G * in->walkR) < in->smCount) in->walkR >>= 1;
     }
-    in->stackDepthMax = std::min(64, std::max(0, envInt("B200_STACK_DEPTH", 12)));
-    if (single) { in->walkVariant = 0; in->stackTail = 0; }     // the experimental walk variants are built for fp64 only
 
     ok = ok && cudaStreamCreateWithFlags(&in->stream, cudaStreamNonBlocking) == cudaSuccess;
     const size_t eigenStride = 2 * (size_t)in->S * in->S + 2 * in->S;
@@ -1750,8 +1664,8 @@ int flushPendingImpl(Instance* in) {
 }
 
 bool fusionPossible(const Instance* in) {
-    return in->fuseSmall && in->matCP > 0 && in->matCP <= 8 && !in->timing && !in->exchangeOn && in->walkVariant == 0 &&
-           in->eigenWalk && in->hMapped != nullptr;
+    return in->fuseSmall && in->matCP > 0 && in->matCP <= 8 && !in->timing && !in->exchangeOn && in->eigenWalk &&
+           in->hMapped != nullptr;
 }
 
 // the whole deferred evaluation as one launch; the caller has checked eligibility
@@ -1892,16 +1806,7 @@ int beagleSetTransitionMatrix(int instance, int matrixIndex, const double* inMat
             {
                 const double v = inMatrix[((size_t)c * in->S + i) * in->S + j];
                 t[matIndex(in, c, i, j)] = v;
-                if (in->matCP) {
-                    double* mm = t.data() + 16 * in->matCP;
-                    mm[(size_t)c * 32 + i * 4 + j] = v;
-                    double* mt = mm + (size_t)in->C * 32;
-                    mt[(size_t)c * 20 + j * 4 + i] = v;
-                    for (int q = 0; q < 4; ++q) {
-                        if (in->S < 4) mt[(size_t)c * 20 + in->S * 4 + q] = q < in->S ? 1.0 : 0.0;
-                        else mt[(size_t)c * 20 + 16 + q] = 1.0;
-                    }
-                } else {
+                if (!in->matCP) {
                     const size_t ld = (size_t)in->Sp + 4, half = (size_t)in->C * in->Sp * in->Sp;
                     t[half + ((size_t)c * in->Sp + i) * ld + j] = v;
                     t[half + (size_t)in->C * in->Sp * ld + ((size_t)c * in->Sp + j) * ld + i] = v;

@@ -29,8 +29,6 @@ struct alignas(16) DevOp {
     const double* scaleRead;
     double* cumScale;
     int pBegin, pEnd;      // pattern range the op applies to (a partition, or [0,P))
-    int srcSlot1, srcSlot2;  // operand-stack slots (4-state stack walk); -1 = read from global
-    int dstSlot;             // operand-stack slot the result is parked in; -1 = none
     int pad_;
 };
 
@@ -40,7 +38,8 @@ struct alignas(16) DevOp {
 //                child (pad_ bit 2 / 3) is its buffer index, i.e. its row of the recipe table, and its two tips are entry
 //                k of a parallel int4 array (child 1: x, y; child 2: z, w) that only k_walk4pv reads
 //   m1/m2      : transition-matrix buffer index;  sw/sr/cum : scale buffer index or -1
-//   slots      : byte0 srcSlot1, byte1 srcSlot2, byte2 dstSlot of the shared-memory operand stack (0xFF = none)
+//   slots      : sibling-stack slots (api.cu::assignStackSlots, read by k_walk4p only): byte0 / byte1 the slot child 1 / 2
+//                is read from, byte2 the slot the result is also written to (0xFF = none)
 //   pad_       : bit 0 = pre-order op, bit 1 = child 1 is the previous op's result (taken from registers),
 //                bit 2 / 3 = child 1 / 2 is a virtual cherry (read by k_walk4pv only, walk4e.cu)
 //   pfA/pfB    : operands of the NEXT op of the walk that are already final in memory, prefetched into L1 while this
@@ -80,7 +79,7 @@ struct CachedPlan {
     // outside the list -- as a virtual cherry (tip1 >= 0, must still be that cherry on a hit) or as stored partials
     std::vector<CherryRef> cherries, external;
     bool readsVirtual = false;                // some op record names a virtual child: needs the eigen form
-    std::vector<int> phaseStart, phaseDepth, phaseSlots;      // phaseSlots: sibling-stack depth per phase
+    std::vector<int> phaseStart, phaseSlots;      // phaseSlots: sibling-stack depth per phase
     int maxWindow = 0;
     long lastUse = 0;
     long hits = 0;
@@ -249,21 +248,17 @@ struct Instance {
     long timedLaunches[T_CLASSES] = {0, 0, 0};
 
     // tuning knobs (environment overridable, see api.cu)
-    size_t walkSmemConfigured = 0, genericSmemConfigured = 0, mmaSmemConfigured[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    size_t genericSmemConfigured = 0, mmaSmemConfigured[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     int walkBlock = 128;
-    int walkVariant = 0;
     std::vector<CachedPlan> planCache;
     int planCacheSize = 4;
     long planClock = 0;
     unsigned long bufferEpoch = 0;     // bumped whenever a buffer changes kind (tip <-> partials) or partitions change
     int reorder = 1;
     int thinR1 = 1;              // thin (latency-bound) phases of the 4-state walk use one pattern group per thread
-    int stackTail = 0;           // operand stack for latency-bound (thin) phases of the 4-state walk (experiment, off)
-    int stackDepthMax = 12;
     int walkMinBlocks = 4;       // __launch_bounds__(128, n) variant of the 4-state walk (4, 5 or 6)
     bool walkMinBlocksSet = false;   // B200_WALK_MINB given explicitly
     int mmaWarps = 4;            // codon-size tensor walk: 4 warps single-buffered (default) or 8 warps double-buffered
-    int tensorR = 2;             // 8-pattern tiles per warp in the 4-state tensor walk (2 or 4)
     int genericMma = 1;          // S > 4: 1 = fp64 tensor-core block walk, 0 = FMA block walk
     int walkR = 4;               // patterns per thread in the 4-state walk (1, 2 or 4)
     int phaseTmin = 4, phaseOversub = 0, phaseSmall = 24;   // phaseSmall: a remainder this short runs as one launch
@@ -283,7 +278,7 @@ void shardedDestroy(Instance* parent);
 cudaError_t launchTransitionMatrices(Instance* in, const int* dProbIdx, const int* dEigenIdx,
                                      const int* dRateSet, const double* dLengths, int count);
 // dSubs[k] = (first op, one-past-last op, first pattern, one-past-last pattern) of subtree walk k
-cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int stackDepth, int maxWindow, bool preOrder);
+cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder);
 // walk4e.cu: eigen-form 4-state walk; eigen = [V (16) | V^-1 (16)]; aligned = every op covers [0, Ppad)
 // new V | V^-1 (32 doubles) for the captured eigen-form walk launches of a graph; any failure = the caller re-captures
 cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphNode_t>& kernelNodes, const double* eigen);

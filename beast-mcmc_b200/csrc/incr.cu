@@ -82,12 +82,6 @@ __device__ __forceinline__ void incrementalBody(const IncArgs& A) {
         if (blockIdx.x == 0) {             // the HBM copies every later launch reads (same layouts as k_transition4)
             double* base = A.mats + (size_t)A.mat[q].prob * A.matStride;
             base[((size_t)j * CP + c) * 4 + i] = acc;
-            double* mm = base + 16 * CP;
-            mm[(size_t)c * 32 + i * 4 + j] = acc;
-            mm[(size_t)c * 32 + 16 + i * 4 + j] = 0.0;
-            double* mt = mm + (size_t)C * 32;
-            mt[(size_t)c * 20 + j * 4 + i] = (j < S) ? acc : ((j == S && i < S) ? 1.0 : 0.0);
-            if (j == 0) mt[(size_t)c * 20 + 16 + i] = (S == 4 && i < S) ? 1.0 : 0.0;
             if (j == 0) A.evecs[((size_t)A.mat[q].prob * CP + c) * 4 + i] = sE[q][c][i];
         }
     }

@@ -3,7 +3,7 @@
 //   k_transition4  : P_c(t) = Evec diag(exp(Eval r_c t)) Ievc, 4-state layouts (updateTransitionMatrices)
 //   k_transition   : the same for the generic layout when k_transition_mma does not apply
 //   k_walk4        : 4-state (nucleotide) partials, WARP-OWNED PATTERN COLUMNS walking the whole
-//                    operation list on-device; per-thread shared-memory operand stack (updatePartials)
+//                    operation list on-device (updatePartials; the eigen-form walks are in walk4e.cu)
 //   k_walk_generic : any state count, BLOCK-OWNED pattern tiles walking the list  (updatePartials)
 //   k_root         : frequency/category integration + log + scalers + weighted reduction
 //   k_scale_accum  : cumulative scale buffers
@@ -12,9 +12,10 @@
 // and states of one site pattern) of a parent depends only on the same column of its children, so a
 // warp (or block) that owns a set of columns can execute the ENTIRE post-order operation list for
 // them without any grid-wide synchronisation: one launch per updatePartials call instead of one per
-// node, and children produced earlier in the same list are read back from shared memory (the
-// operand stack), not from HBM.  The only mandatory HBM traffic is the write of every destination
-// buffer (BEAST needs them for later incremental updates) plus tips and pre-existing siblings.
+// node, and children produced earlier in the same list are taken from registers (the previous op's
+// result), the sibling stack in shared memory (walk4e.cu) or L2, not from HBM.  The only mandatory
+// HBM traffic is the write of every destination buffer (BEAST needs them for later incremental
+// updates) plus tips and pre-existing siblings.
 #include "engine.h"
 #include "walk4.cuh"
 
@@ -104,8 +105,6 @@ __global__ void k_transition(const double* __restrict__ eigenBase, size_t eigenS
 // Writes, per (branch, category):
 //   [j][CP][i]    : row j of all categories is one 128-byte line (k_walk4*, k_walk4e matrix form, getTransitionMatrix)
 //   [matrix][CP][4] spectrum exp(lambda_k r_c t) for the eigen-form walk (walk4e.cu)
-//   Mpad[c][8][4] : B fragment of k_walk4t, lane (g,t) reads [g][t]; rows g >= 4 stay zero
-//   MTg [c][5][4] : column s of P for a compact tip in state s, plus the gap column s == S = (1,..,1,0..)
 constexpr int kTransition4Block = 256;
 __global__ void __launch_bounds__(kTransition4Block)
 k_transition4(const double* __restrict__ eigenBase, size_t eigenStride, int S, int C, int CP, int complexForm,
@@ -179,28 +178,16 @@ k_transition4(const double* __restrict__ eigenBase, size_t eigenStride, int S, i
             }
         }
     }
-    double p[2][2], g[2][2];                                      // the tile after abs(); the same as MTg entries [j][i]
+    double p[2][2];                                               // the tile after abs()
 #pragma unroll
     for (int a = 0; a < 2; ++a)
 #pragma unroll
-        for (int t = 0; t < 2; ++t) {
-            const int i = i0 + a, j = j0 + t;
-            p[a][t] = (i < S && j < S) ? fabs(acc[a][t]) : 0.0;
-            g[a][t] = (j < S) ? p[a][t] : ((j == S && i < S) ? 1.0 : 0.0);
-        }
+        for (int t = 0; t < 2; ++t) p[a][t] = (i0 + a < S && j0 + t < S) ? fabs(acc[a][t]) : 0.0;
     const int mat = sProb[r];
     double* base = matBase + (size_t)mat * matStride;
-    double* mm = base + 16 * (size_t)CP + (size_t)c * 32;
-    double* mt = base + 16 * (size_t)CP + (size_t)C * 32 + (size_t)c * 20;
 #pragma unroll
-    for (int t = 0; t < 2; ++t) {
-        // row j0 + t of [j][CP][i] and of MTg, entries i0, i0 + 1; row i0 + t of Mpad, entries j0, j0 + 1
+    for (int t = 0; t < 2; ++t)   // row j0 + t of [j][CP][i], entries i0, i0 + 1
         *reinterpret_cast<double2*>(base + ((size_t)(j0 + t) * CP + c) * 4 + i0) = make_double2(p[0][t], p[1][t]);
-        *reinterpret_cast<double2*>(mt + (j0 + t) * 4 + i0) = make_double2(g[0][t], g[1][t]);
-        *reinterpret_cast<double2*>(mm + (i0 + t) * 4 + j0) = make_double2(p[t][0], p[t][1]);
-        *reinterpret_cast<double2*>(mm + 16 + 8 * t + 2 * k) = make_double2(0.0, 0.0);
-    }
-    mt[16 + k] = S == 4 ? 1.0 : 0.0;
     evecBase[((size_t)mat * CP + c) * 4 + k] = k < S ? ec : 0.0;
 }
 
@@ -230,13 +217,6 @@ k_combine_matrices(double* __restrict__ matBase, size_t matStride, int S, int Sp
             double* padded = R + (size_t)C * Sp * Sp;
             padded[((size_t)c * Sp + i) * ld + j] = v;                                  // M[c][i][.]
             padded[(size_t)C * Sp * ld + ((size_t)c * Sp + j) * ld + i] = v;            // MT[c][j][.]
-        } else {
-            double* mm = R + 16 * matCP;                                                // tensor-variant copies (k_walk4t)
-            mm[(size_t)c * 32 + i * 4 + j] = v;
-            mm[(size_t)c * 32 + 16 + i * 4 + j] = 0.0;
-            double* mt = mm + (size_t)C * 32;
-            mt[(size_t)c * 20 + j * 4 + i] = (j < S) ? v : ((j == S && i < S) ? 1.0 : 0.0);
-            if (j == 0) mt[(size_t)c * 20 + 16 + i] = (S == 4 && i < S) ? 1.0 : 0.0;
         }
     }
 }
@@ -363,9 +343,7 @@ cudaError_t launchTransitionMatrices(Instance* in, const int* dProbIdx, const in
 //   * op record: 64 B, warp-uniform, four 128-bit loads; record k+2 is prefetched to L1, record k+1 read after the
 //     arithmetic (R > 1) or one op ahead (R = 1); it also names what the NEXT op will read (look-ahead prefetch)
 //   * matrices : layout [j][CP][i] -> row j of all categories is one 128-byte line, 4 loads per child
-//   * the child produced by the previous op of the walk: taken from the thread's own registers (op flag bit 1);
-//     optional variant (B200_WALK_VARIANT=1): a per-thread operand stack in shared memory for every such child,
-//     laid out [slot][half][thread] so every LDS.128/STS.128 is bank-conflict free
+//   * the child produced by the previous op of the walk: taken from the thread's own registers (op flag bit 1)
 //   * tip states: one byte per pattern; their line is prefetched one op ahead
 struct Mat4 { double r[4][4]; };     // r[j][i] = P[i][j] of this thread's category
 
@@ -386,10 +364,9 @@ __device__ __forceinline__ void applyMat(const Mat4& M, const double (&x)[4], do
 // matrices in registers and re-uses them for R patterns (R = patterns per thread, strided by G so
 // that every load/store instruction still covers 8 consecutive patterns = 256 contiguous bytes).
 // one child's contribution for the R patterns of this thread: y[r][i] (*)= sum_j P[i][j] x_r[j]
-template <typename T, int CP, int R, bool STACK, bool FIRST>
-__device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matIdx, int slot, int moff, size_t off0,
-                                          int p0, bool catValid, int pBegin, int pEnd, const double2* stackMem,
-                                          int nthreads, double (&y)[R][4]) {
+template <typename T, int CP, int R, bool FIRST>
+__device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matIdx, int moff, size_t off0,
+                                          int p0, bool catValid, int pBegin, int pEnd, double (&y)[R][4]) {
     constexpr int G = 32 / CP;
     const int S = A.S;
     const double* m = A.mats + (size_t)matIdx * A.matStride + moff;
@@ -418,13 +395,8 @@ __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matI
             const int p = p0 + r * G;
             const bool active = catValid && p >= pBegin && p < pEnd;
             double x[4], v[4];
-            if (STACK && slot != 0xFF) {
-                double2 lo = stackMem[((slot * R + r) * 2 + 0) * nthreads + threadIdx.x];
-                double2 hi = stackMem[((slot * R + r) * 2 + 1) * nthreads + threadIdx.x];
-                x[0] = lo.x; x[1] = lo.y; x[2] = hi.x; x[3] = hi.y;
-            } else if (active) {
-                loadCell(xg + (size_t)r * G * 4, x);
-            } else { x[0] = x[1] = x[2] = x[3] = 0.0; }
+            if (active) loadCell(xg + (size_t)r * G * 4, x);
+            else { x[0] = x[1] = x[2] = x[3] = 0.0; }
             applyMat(M, x, v);
 #pragma unroll
             for (int i = 0; i < 4; ++i) y[r][i] = FIRST ? v[i] : y[r][i] * v[i];
@@ -432,11 +404,9 @@ __device__ __forceinline__ void childTerm(const WalkArgs& A, int child, int matI
     }
 }
 
-template <typename T, int CP, int R, bool STACK, bool PRE>
+template <typename T, int CP, int R, bool PRE>
 __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
-    static_assert(sizeof(T) == 8 || !STACK, "the operand-stack variant is built for fp64 partials only");
     constexpr int G = 32 / CP;
-    extern __shared__ double2 stackMem[];
     const int lane = threadIdx.x & 31;
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int c = lane / G;
@@ -448,7 +418,6 @@ __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
     const int cc = catValid ? c : 0;
     const size_t off0 = ((size_t)cc * A.Ppad + p0) * 4;
     const int moff = cc * 4;
-    const int nthreads = blockDim.x;
     const int last = range.y - 1;
 
     Op4 cur = loadOp(A.ops + range.x);
@@ -462,31 +431,28 @@ __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
         Op4 nxt;
         if (R == 1) nxt = loadOp(A.ops + min(k + 1, last));
         else if (lane == 0) prefetchL1(A.ops + min(k + 2, last));
-        const int s1 = cur.slots & 0xFF, s2 = (cur.slots >> 8) & 0xFF, sd = (cur.slots >> 16) & 0xFF;
-        if (!STACK) {
-            // look-ahead: the NEXT op's memory operands (never this op's destination) start their trip to L1 now,
-            // so that its loads find them there when this op is done
+        // look-ahead: the NEXT op's memory operands (never this op's destination) start their trip to L1 now,
+        // so that its loads find them there when this op is done
 #pragma unroll
-            for (int w = 0; w < 2; ++w) {
-                const int pf = w == 0 ? cur.pfA : cur.pfB;
-                if (pf == 0) continue;
-                if (pf & 1) {
-                    const uint8_t* t = A.states + (size_t)(pf >> 1) * A.Ppad + p0;
-                    if ((lane % G) == 0 && c == 0) prefetchL1(t);          // G*R consecutive bytes: one line
-                } else if (catValid) {
-                    const T* xg = static_cast<const T*>(A.partials) + (size_t)((pf >> 1) - 1) * A.stride + off0;
+        for (int w = 0; w < 2; ++w) {
+            const int pf = w == 0 ? cur.pfA : cur.pfB;
+            if (pf == 0) continue;
+            if (pf & 1) {
+                const uint8_t* t = A.states + (size_t)(pf >> 1) * A.Ppad + p0;
+                if ((lane % G) == 0 && c == 0) prefetchL1(t);          // G*R consecutive bytes: one line
+            } else if (catValid) {
+                const T* xg = static_cast<const T*>(A.partials) + (size_t)((pf >> 1) - 1) * A.stride + off0;
 #pragma unroll
-                    for (int r = 0; r < R; ++r)
-                        if (p0 + r * G < A.Ppad) prefetchL1(xg + (size_t)r * G * 4);
-                }
-            }
-            if (lane < 8) {
-                const int mi = lane < 4 ? cur.pfM1 : cur.pfM2;
-                if (mi >= 0) prefetchL1(A.mats + (size_t)mi * A.matStride + (lane & 3) * 4 * CP);
+                for (int r = 0; r < R; ++r)
+                    if (p0 + r * G < A.Ppad) prefetchL1(xg + (size_t)r * G * 4);
             }
         }
+        if (lane < 8) {
+            const int mi = lane < 4 ? cur.pfM1 : cur.pfM2;
+            if (mi >= 0) prefetchL1(A.mats + (size_t)mi * A.matStride + (lane & 3) * 4 * CP);
+        }
         if (!PRE) {
-            if (!STACK && (cur.pad_ & 2)) {
+            if (cur.pad_ & 2) {
                 // the first child is what this very thread produced for the previous op of the walk: take it from
                 // registers (no store -> L2 -> load round trip, one partial less through the LSU)
                 Mat4 M;
@@ -499,16 +465,16 @@ __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
                     for (int i = 0; i < 4; ++i) d[r][i] = v[i];
                 }
             } else {
-                childTerm<T, CP, R, STACK, true>(A, cur.c1, cur.m1, s1, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
+                childTerm<T, CP, R, true>(A, cur.c1, cur.m1, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, d);
             }
-            childTerm<T, CP, R, STACK, false>(A, cur.c2, cur.m2, s2, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, d);
+            childTerm<T, CP, R, false>(A, cur.c2, cur.m2, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, d);
         } else {
             // pre-order op: q = pre[parent] (*) (M_sib post[sib]) at the parent, then down the node's own branch
             // with the transposed matrix: pre[node][j] = sum_i q[i] M_node[i][j]
             // (depth-first order inside a subtree walk: when this node is the first child of the previous op's node,
             // pre[parent] is still in d -- flag bit 1 -- and is not re-read)
             double v[R][4];
-            childTerm<T, CP, R, false, true>(A, cur.c2, cur.m2, 0xFF, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, stackMem, nthreads, v);
+            childTerm<T, CP, R, true>(A, cur.c2, cur.m2, moff, off0, p0, catValid, cur.pBegin, cur.pEnd, v);
             Mat4 M1;
             loadMat<CP>(A.mats + (size_t)cur.m1 * A.matStride + moff, M1);
             const T* xg = static_cast<const T*>(A.partials) + (size_t)cur.c1 * A.stride + off0;
@@ -558,46 +524,37 @@ __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
             }
             roundCell<T>(d[r]);
             if (active) storeCell(dg + (size_t)r * G * 4, d[r]);
-            if (STACK && sd != 0xFF) {
-                stackMem[((sd * R + r) * 2 + 0) * nthreads + threadIdx.x] = make_double2(d[r][0], d[r][1]);
-                stackMem[((sd * R + r) * 2 + 1) * nthreads + threadIdx.x] = make_double2(d[r][2], d[r][3]);
-            }
         }
         cur = nxt;
     }
 }
 
-template <int CP, int R, bool STACK, int MINB, bool PRE>
+template <int CP, int R, int MINB, bool PRE>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4(const WalkArgs A) {
-    walk4Body<double, CP, R, STACK, PRE>(A);
+    walk4Body<double, CP, R, PRE>(A);
 }
 
-// fp32 partials storage (PRECISION_SINGLE); no operand-stack variant
+// fp32 partials storage (PRECISION_SINGLE)
 template <int CP, int R, int MINB, bool PRE>
 __global__ void __launch_bounds__(128, MINB)
 k_walk4s(const WalkArgs A) {
-    walk4Body<float, CP, R, false, PRE>(A);
+    walk4Body<float, CP, R, PRE>(A);
 }
 
-template <int CP, int R, bool STACK, int MINB, bool PRE = false>
-static cudaError_t launchWalk4K(Instance* in, const WalkArgs& A, dim3 grid, size_t smem) {
-    if (in->single) {                  // the stack variant never runs on a single instance (walkVariant = stackTail = 0)
-        if constexpr (!STACK && CP <= 8) k_walk4s<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
+template <int CP, int R, int MINB, bool PRE = false>
+static cudaError_t launchWalk4K(Instance* in, const WalkArgs& A, dim3 grid) {
+    if (in->single) {
+        if constexpr (CP <= 8) k_walk4s<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
         else return cudaErrorInvalidValue;
         return cudaGetLastError();
     }
-    if (smem > 0 && smem > in->walkSmemConfigured) {
-        cudaError_t e = cudaFuncSetAttribute(k_walk4<CP, R, STACK, MINB, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        in->walkSmemConfigured = smem;
-    }
-    k_walk4<CP, R, STACK, MINB, PRE><<<grid, 128, smem, in->stream>>>(A);
+    k_walk4<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
 template <int CP, int R>
-static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int stackDepth, int maxWindow, bool preOrder) {
+static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
     constexpr int G = 32 / CP;
     const int warps = (maxWindow + G * R - 1) / (G * R);
     dim3 grid((warps + 3) / 4, nSubs);
@@ -605,184 +562,36 @@ static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs
     A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
     A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
     A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
-    A.matStride = in->matStride; A.matMmaOffset = 16 * in->matCP;
-    if (preOrder) return launchWalk4K<CP, R, false, 4, true>(in, A, grid, 0);
-    if (stackDepth > 0) return launchWalk4K<CP, R, true, 4>(in, A, grid, (size_t)stackDepth * 32 * R * 128);
-    if (in->walkMinBlocks >= 6) return launchWalk4K<CP, R, false, 6>(in, A, grid, 0);
-    if (in->walkMinBlocks == 5) return launchWalk4K<CP, R, false, 5>(in, A, grid, 0);
-    if (in->walkMinBlocks == 3) return launchWalk4K<CP, R, false, 3>(in, A, grid, 0);
-    return launchWalk4K<CP, R, false, 4>(in, A, grid, 0);
-}
-
-// ---------------------------------------------------------------------------------------------
-// 4-state walk on the FP64 tensor pipe (DMMA m8n8k4)  --  B200_WALK_VARIANT=2
-// ---------------------------------------------------------------------------------------------
-// D[p][i] = sum_j X[p][j] * P[i][j]  as one mma.sync.m8n8k4.f64 per (8 patterns, category, child):
-//   A fragment = child partials  [8 patterns][4 states]   lane (g,t) <- X[p0+g][t]     (256 contiguous bytes / warp)
-//   B fragment = transition rows [4 (j)][8 (i)]            lane (g,t) <- Mpad[g][t]     (256 contiguous bytes, rows >= 4 zero)
-//   D fragment                    [8 patterns][8 (i)]      lane (g,t) -> i = 2t,2t+1 of pattern g (meaningful for t < 2)
-// wgmma has no fp64 kind, so the fp64 tensor path on sm_90a is mma.sync (SASS DMMA.8x8x4).
-// The matrix reaches the register file ONCE per warp (8 B/lane) instead of once per thread (128 B/lane),
-// which is what saturates the LSU->RF path of the FMA kernel.  Everything is arranged so that loads need
-// no predicates: pattern rows are padded to 32, gap tips read a ones-column, B rows 4..7 are stored zeros;
-// only stores (and scale-factor writes) are masked.  Warp = C categories x R tiles of 8 patterns.
-__device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double b) {
-    asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%4,%5};"
-        : "=d"(d0), "=d"(d1) : "d"(a), "d"(b), "d"(0.0), "d"(0.0));
-}
-
-template <int C, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
-k_walk4t(const WalkArgs A) {
-    const int lane = threadIdx.x & 31;
-    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int4 range = __ldg(A.subs + blockIdx.y);
-    if (range.z + warp * (8 * R) >= range.w) return;
-    const int g = lane >> 2, t = lane & 3;
-    const int pBase = range.z + warp * (8 * R) + g;        // pattern of tile r: pBase + 8 r   (always < Ppad)
-    const size_t mstride = A.matStride;
-    const size_t catStride = (size_t)A.Ppad * 4;
-    const size_t cellOff = (size_t)pBase * 4;
-    const int last = range.y - 1;
-    const double* matB = A.mats + A.matMmaOffset + lane;                    // Mpad[c][g][t] = + c*32
-    const double* matT = A.mats + A.matMmaOffset + C * 32 + 2 * (t & 1);     // MTg[c][s][2t..] = + c*20 + s*4
-
-    Op4 cur = loadOp(A.ops + range.x);
-    for (int k = range.x; k <= last; ++k) {
-        const Op4 nxt = loadOp(A.ops + min(k + 1, last));
-        double y[C][R][2];
-#pragma unroll
-        for (int child = 0; child < 2; ++child) {
-            const int cb = child == 0 ? cur.c1 : cur.c2;
-            const size_t moff = (size_t)(child == 0 ? cur.m1 : cur.m2) * mstride;
-            if (cb >= 0) {
-                const double* x = static_cast<const double*>(A.partials) + (size_t)cb * A.stride + cellOff + t;
-                double b[C];
-#pragma unroll
-                for (int c = 0; c < C; ++c) b[c] = __ldg(matB + moff + c * 32);
-#pragma unroll
-                for (int c = 0; c < C; ++c) {
-#pragma unroll
-                    for (int r = 0; r < R; ++r) {
-                        double a, d0, d1;
-                        asm volatile("ld.global.f64 %0, [%1];" : "=d"(a) : "l"(x + c * catStride + r * 32) : "memory");
-                        dmma884(d0, d1, a, b[c]);
-                        if (child == 0) { y[c][r][0] = d0; y[c][r][1] = d1; }
-                        else { y[c][r][0] *= d0; y[c][r][1] *= d1; }
-                    }
-                }
-            } else {
-                const uint8_t* st = A.states + (size_t)(-cb - 1) * A.Ppad + pBase;
-#pragma unroll
-                for (int r = 0; r < R; ++r) {
-                    const int s = (int)__ldg(st + 8 * r);                    // gap/unknown is stored as S -> ones column
-                    const double* col = matT + moff + s * 4;
-#pragma unroll
-                    for (int c = 0; c < C; ++c) {
-                        const double2 v = __ldg(reinterpret_cast<const double2*>(col + c * 20));
-                        if (child == 0) { y[c][r][0] = v.x; y[c][r][1] = v.y; }
-                        else { y[c][r][0] *= v.x; y[c][r][1] *= v.y; }
-                    }
-                }
-            }
-        }
-        // ---- fused rescale (AbstractLikelihoodCore.java:406-442, unconditional as in BEAGLE) ---------
-        if (cur.sw >= 0 || cur.sr >= 0) {
-#pragma unroll
-            for (int r = 0; r < R; ++r) {
-                const int p = pBase + 8 * r;
-                const bool act = p >= cur.pBegin && p < cur.pEnd;
-                double f;
-                if (cur.sw >= 0) {
-                    double m = 0.0;
-#pragma unroll
-                    for (int c = 0; c < C; ++c) m = fmax(m, fmax(y[c][r][0], y[c][r][1]));
-                    if (t >= 2) m = 0.0;                                     // lanes t >= 2 carry no states
-                    m = fmax(m, __shfl_xor_sync(0xffffffffu, m, 1));
-                    m = fmax(m, __shfl_xor_sync(0xffffffffu, m, 2));
-                    if (m == 0.0) m = 1.0;
-                    f = m;
-                    if (act && t == 0) {
-                        A.scale[(size_t)cur.sw * A.Ppad + p] = A.logScalers ? log(m) : m;
-                    }
-                } else {
-                    f = act ? A.scale[(size_t)cur.sr * A.Ppad + p] : 1.0;
-                    if (A.logScalers) f = exp(f);
-                }
-                const double inv = 1.0 / f;
-#pragma unroll
-                for (int c = 0; c < C; ++c) { y[c][r][0] *= inv; y[c][r][1] *= inv; }
-            }
-        }
-        // ---- store: lanes t < 2 own states 2t, 2t+1 (16 B) of pattern g ---------------------------
-        {
-            double* dst = static_cast<double*>(A.partials) + (size_t)cur.dest * A.stride + cellOff + 2 * t;
-#pragma unroll
-            for (int r = 0; r < R; ++r) {
-                const int p = pBase + 8 * r;
-                if (t < 2 && p >= cur.pBegin && p < cur.pEnd) {
-#pragma unroll
-                    for (int c = 0; c < C; ++c)
-                        asm volatile("st.global.v2.f64 [%0], {%1,%2};" :: "l"(dst + c * catStride + r * 32),
-                                     "d"(y[c][r][0]), "d"(y[c][r][1]) : "memory");
-                }
-            }
-        }
-        __syncwarp();          // the next op may read (through other lanes of this warp) what was just stored
-        cur = nxt;
-    }
-}
-
-template <int C, int R>
-static cudaError_t launchWalk4Tensor(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow) {
-    const int warps = (maxWindow + 8 * R - 1) / (8 * R);
-    dim3 grid((warps + 3) / 4, nSubs);
-    WalkArgs A;
-    A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
-    A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
-    A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
-    A.matStride = in->matStride; A.matMmaOffset = 16 * in->matCP;
-    if (in->walkMinBlocks >= 6) k_walk4t<C, R, 6><<<grid, 128, 0, in->stream>>>(A);
-    else k_walk4t<C, R, 4><<<grid, 128, 0, in->stream>>>(A);
-    return cudaGetLastError();
-}
-
-// exact category counts only (fully unrolled); anything else stays on the FMA kernel
-static bool walk4TensorSupported(const Instance* in) { return in->C == 1 || in->C == 2 || in->C == 4 || in->C == 8; }
-
-static cudaError_t launchWalk4Mma(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow) {
-    const bool r4 = in->tensorR >= 4;
-    switch (in->C) {
-        case 1: return r4 ? launchWalk4Tensor<1, 4>(in, dOps, dSubs, nSubs, maxWindow) : launchWalk4Tensor<1, 2>(in, dOps, dSubs, nSubs, maxWindow);
-        case 2: return r4 ? launchWalk4Tensor<2, 4>(in, dOps, dSubs, nSubs, maxWindow) : launchWalk4Tensor<2, 2>(in, dOps, dSubs, nSubs, maxWindow);
-        case 4: return r4 ? launchWalk4Tensor<4, 4>(in, dOps, dSubs, nSubs, maxWindow) : launchWalk4Tensor<4, 2>(in, dOps, dSubs, nSubs, maxWindow);
-        default: return launchWalk4Tensor<8, 2>(in, dOps, dSubs, nSubs, maxWindow);
-    }
+    A.matStride = in->matStride;
+    if (preOrder) return launchWalk4K<CP, R, 4, true>(in, A, grid);
+    if (in->walkMinBlocks >= 6) return launchWalk4K<CP, R, 6>(in, A, grid);
+    if (in->walkMinBlocks == 5) return launchWalk4K<CP, R, 5>(in, A, grid);
+    if (in->walkMinBlocks == 3) return launchWalk4K<CP, R, 3>(in, A, grid);
+    return launchWalk4K<CP, R, 4>(in, A, grid);
 }
 
 template <int CP>
-static cudaError_t launchWalk4T(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int stackDepth, int maxWindow, bool preOrder) {
+static cudaError_t launchWalk4T(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
     // a thin phase (few walks in flight) is latency-bound: one pattern group per thread gives 4x the warps per op
     const long walks = (long)nSubs * ((maxWindow + (32 / CP) * in->walkR - 1) / ((32 / CP) * in->walkR));
-    if (in->thinR1 && stackDepth == 0 && walks < (long)in->smCount * 8)
-        return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
+    if (in->thinR1 && walks < (long)in->smCount * 8)
+        return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
     switch (in->walkR) {
-        case 4: return launchWalk4R<CP, 4>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        case 2: return launchWalk4R<CP, 2>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        default: return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
+        case 4: return launchWalk4R<CP, 4>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        case 2: return launchWalk4R<CP, 2>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        default: return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
     }
 }
 
-cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int stackDepth, int maxWindow, bool preOrder) {
+cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
     if (nSubs <= 0) return cudaSuccess;
-    if (in->walkVariant == 2 && !preOrder && walk4TensorSupported(in)) return launchWalk4Mma(in, dOps, dSubs, nSubs, maxWindow);
     switch (in->matCP) {
-        case 1: return launchWalk4T<1>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        case 2: return launchWalk4T<2>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        case 4: return launchWalk4T<4>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        case 8: return launchWalk4T<8>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        case 16: return launchWalk4T<16>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
-        default: return launchWalk4T<32>(in, dOps, dSubs, nSubs, stackDepth, maxWindow, preOrder);
+        case 1: return launchWalk4T<1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        case 2: return launchWalk4T<2>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        case 4: return launchWalk4T<4>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        case 8: return launchWalk4T<8>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        case 16: return launchWalk4T<16>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+        default: return launchWalk4T<32>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
     }
 }
 

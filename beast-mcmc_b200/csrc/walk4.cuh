@@ -64,7 +64,6 @@ struct WalkArgs {
     double* scale;             // [buffer][Ppad]
     int S, C, Ppad, logScalers;
     size_t matStride;          // elements per matrix buffer
-    int matMmaOffset;          // offset of the [c][i][j] + [c][j][i] copies inside a matrix buffer
     // eigen-form walk (walk4e.cu): per-branch spectra exp(lambda_k r_c t) [matrix][CP][4] in HBM, and the ONE eigen system
     // of the list by value -- kernel parameters live in the constant bank, so V / V^-1 cost neither registers nor LSU
     // traffic (DFMA takes them as uniform-register operands)

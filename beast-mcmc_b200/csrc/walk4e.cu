@@ -728,7 +728,7 @@ cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int n
     A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
     A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
     A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
-    A.matStride = in->matStride; A.matMmaOffset = 16 * in->matCP;
+    A.matStride = in->matStride;
     A.evecs = in->dEvec;
     A.recipes = in->dRecipe;
     A.virtTips = dVirtTips;

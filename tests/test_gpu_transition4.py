@@ -1,9 +1,8 @@
 """The 4-state transition-matrix kernel (k_transition4: every instance with S <= 4 and at most 32 categories).
 
 Each case checks getTransitionMatrix of every branch against a numpy restatement of BaseSubstitutionModel.java:206-241 and
-ComplexColtEigenSystem.java:71-139, then runs full evaluations against the oracle. The evaluations read the other copies
-the kernel writes: the spectra (eigen-form walk, real systems), the [j][CP][i] block (matrix-form walk) and the tensor
-walk's Mpad / MTg copies (B200_WALK_VARIANT=2, C in {1, 2, 4, 8}).
+ComplexColtEigenSystem.java:71-139, then runs full evaluations against the oracle. The evaluations read what else the
+kernel writes: the spectra (eigen-form walk, real systems) and the [j][CP][i] block (matrix-form walk).
 """
 import numpy as np
 import pytest
@@ -135,14 +134,14 @@ def test_matrices_match_restatement(S, C, kind):
 @pytest.mark.parametrize("S,C,kind", CASES)
 def test_evaluation_matches_oracle(S, C, kind, monkeypatch):
     """One full evaluation per route against the oracle: the default walk (eigen form on a real system, matrix form on a
-    complex one), the matrix-form walk, and the tensor walk (its Mpad / MTg copies; other C fall back to the FMA walk)."""
+    complex one) and the matrix-form walk."""
     tree, pats, model, site = H.synthetic_case(24, 200, categories=C, seed=20 + S + C, stateCount=S, rootHeight=0.5)
     if kind == "complex":
         model = _ComplexModel(S, 7 + S)
     o = tdl.BeagleDataLikelihoodDelegate(tree, pats, model, site, H.oracle_factory(report_flags=0),
                                          rescalingScheme=tdl.PartialsRescalingScheme.NONE)
     want = tdl.TreeDataLikelihood(o, tree).getLogLikelihood()
-    for env in ({}, {"B200_EIGEN_WALK": "0"}, {"B200_WALK_VARIANT": "2"}):
+    for env in ({}, {"B200_EIGEN_WALK": "0"}):
         with monkeypatch.context() as mp:
             for k, v in env.items():
                 mp.setenv(k, v)

@@ -1,14 +1,14 @@
 #!/bin/bash
 # Kernel-variant sweep for the 4-state walk (run on the GPU box): one bench line per setting.
-# columns: variant(0 global,1 stack) reorder minBlocks stackDepth phaseT(0=auto) R(patterns/thread) Tmin oversub
+# columns: reorder minBlocks phaseT(0=auto) R(patterns/thread) Tmin oversub
 mkdir -p gpurun_out
 python bench.py --steps 5 --warmup 3 --no-cpu-baseline > /dev/null 2>&1   # builds the alignment cache
-CFGS=${CFGS:-"0 1 5 12 0 2 4 3;0 1 5 12 0 2 4 2;0 1 5 12 0 2 8 2;0 1 4 12 0 4 4 2;0 1 5 12 0 2 16 2;0 1 5 12 0 2 4 1"}
+CFGS=${CFGS:-"1 5 0 2 4 3;1 5 0 2 4 2;1 5 0 2 8 2;1 4 0 4 4 2;1 5 0 2 16 2;1 5 0 2 4 1"}
 IFS=';' read -ra LIST <<< "$CFGS"
 for cfg in "${LIST[@]}"; do
   set -- $cfg
-  echo "variant=$1 reorder=$2 minb=$3 depth=$4 phaseT=$5 R=$6 Tmin=$7 oversub=$8"
-  B200_WALK_VARIANT=$1 B200_REORDER=$2 B200_WALK_MINB=$3 B200_STACK_DEPTH=$4 B200_PHASE_T=$5 B200_WALK_R=$6 B200_PHASE_TMIN=$7 B200_PHASE_OVERSUB=$8 \
+  echo "reorder=$1 minb=$2 phaseT=$3 R=$4 Tmin=$5 oversub=$6"
+  B200_REORDER=$1 B200_WALK_MINB=$2 B200_PHASE_T=$3 B200_WALK_R=$4 B200_PHASE_TMIN=$5 B200_PHASE_OVERSUB=$6 \
     python bench.py --steps ${STEPS:-100} --warmup 5 --no-cpu-baseline $BENCH_ARGS 2>&1 | python -c "
 import sys, json
 for l in sys.stdin:
