@@ -1210,8 +1210,6 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->eigenKind.assign(std::max(1, in->nEigen), 0);
     in->hEigen.assign((size_t)std::max(1, in->nEigen) * 36, 0.0);
     in->eigenWalk = envInt("B200_EIGEN_WALK", 1);
-    in->tipMode = envInt("B200_TIP_MODE", 3);
-    in->thinTipMode = envInt("B200_THIN_TIP_MODE", in->tipMode);
     in->virtualCherries = envInt("B200_VIRTUAL_CHERRIES", 1);
     in->walkBlock = 128;
     in->reorder = envInt("B200_REORDER", 1);
@@ -1229,8 +1227,6 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->phaseTmin = std::max(1, envInt("B200_PHASE_TMIN", 4));
     in->phaseSmall = envInt("B200_PHASE_SMALL", 24);
     in->phaseOversub = std::max(0, envInt("B200_PHASE_OVERSUB", 0));      // 0 = by subtree width (see wantSubsFor)
-    in->walkMinBlocks = envInt("B200_WALK_MINB", 4);
-    in->walkMinBlocksSet = getenv("B200_WALK_MINB") != nullptr;
     in->genericMma = envInt("B200_GENERIC_MMA", 1);
     in->mmaWarps = envInt("B200_MMA_WARPS", 4) == 8 ? 8 : 4;     // 8 = 256-thread blocks with cp.async double buffering
     // the SM count sizes the walk below: query the device first
@@ -1238,7 +1234,7 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     bool ok = cudaGetDeviceProperties(&prop, in->device) == cudaSuccess;
     if (ok) { in->smCount = prop.multiProcessorCount; in->maxSmemOptin = prop.sharedMemPerBlockOptin; }
     in->walkR = envInt("B200_WALK_R", 4);
-    if (in->walkR != 1 && in->walkR != 2 && in->walkR != 4 && in->walkR != 8) in->walkR = 4;
+    if (in->walkR != 1 && in->walkR != 2 && in->walkR != 4) in->walkR = 4;
     if (getenv("B200_WALK_R") == nullptr && in->matCP > 0) {
         // patterns per thread: as many as still leave >= 1 warp per SM inside ONE subtree walk (the phases supply the rest of
         // the parallelism: measured on the 6000-pattern Makona-like set, 25 subtrees per launch: R = 4 0.273 ms, R = 2 0.340 ms)

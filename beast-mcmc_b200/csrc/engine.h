@@ -179,8 +179,6 @@ struct Instance {
     std::vector<char> eigenKind;              // any S: 0 = slot never set, 1 = real, 2 = holds complex pairs
     std::vector<double> hEigen;               // [nEigen][32]: V | V^-1 padded to 4 x 4 (host copy, by value into the launch)
     int eigenWalk = 1;                        // B200_EIGEN_WALK: 0 = always the matrix-form kernel
-    int tipMode = 2;                          // B200_TIP_MODE: compact tips by contraction (0), P column from global (1), shared-memory column table (2)
-    int thinTipMode = 3;                     // the same choice for thin (R = 1) phases (B200_THIN_TIP_MODE)
     // virtual cherries (B200_VIRTUAL_CHERRIES, 4-state CP <= 8): per buffer the tips of the cherry it holds (-1 = real
     // partials) and whether its partials have been written too; recipe rows [buffer][2][16 * CP]
     int virtualCherries = 1;
@@ -256,8 +254,6 @@ struct Instance {
     unsigned long bufferEpoch = 0;     // bumped whenever a buffer changes kind (tip <-> partials) or partitions change
     int reorder = 1;
     int thinR1 = 1;              // thin (latency-bound) phases of the 4-state walk use one pattern group per thread
-    int walkMinBlocks = 4;       // __launch_bounds__(128, n) variant of the 4-state walk (4, 5 or 6)
-    bool walkMinBlocksSet = false;   // B200_WALK_MINB given explicitly
     int mmaWarps = 4;            // codon-size tensor walk: 4 warps single-buffered (default) or 8 warps double-buffered
     int genericMma = 1;          // S > 4: 1 = fp64 tensor-core block walk, 0 = FMA block walk
     int walkR = 4;               // patterns per thread in the 4-state walk (1, 2 or 4)

@@ -529,27 +529,27 @@ __device__ __forceinline__ void walk4Body(const WalkArgs& A) {
     }
 }
 
-template <int CP, int R, int MINB, bool PRE>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R, bool PRE>
+__global__ void __launch_bounds__(128, 4)
 k_walk4(const WalkArgs A) {
     walk4Body<double, CP, R, PRE>(A);
 }
 
 // fp32 partials storage (PRECISION_SINGLE)
-template <int CP, int R, int MINB, bool PRE>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R, bool PRE>
+__global__ void __launch_bounds__(128, 4)
 k_walk4s(const WalkArgs A) {
     walk4Body<float, CP, R, PRE>(A);
 }
 
-template <int CP, int R, int MINB, bool PRE = false>
+template <int CP, int R, bool PRE>
 static cudaError_t launchWalk4K(Instance* in, const WalkArgs& A, dim3 grid) {
     if (in->single) {
-        if constexpr (CP <= 8) k_walk4s<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
+        if constexpr (CP <= 8) k_walk4s<CP, R, PRE><<<grid, 128, 0, in->stream>>>(A);
         else return cudaErrorInvalidValue;
         return cudaGetLastError();
     }
-    k_walk4<CP, R, MINB, PRE><<<grid, 128, 0, in->stream>>>(A);
+    k_walk4<CP, R, PRE><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
@@ -563,11 +563,8 @@ static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs
     A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
     A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
     A.matStride = in->matStride;
-    if (preOrder) return launchWalk4K<CP, R, 4, true>(in, A, grid);
-    if (in->walkMinBlocks >= 6) return launchWalk4K<CP, R, 6>(in, A, grid);
-    if (in->walkMinBlocks == 5) return launchWalk4K<CP, R, 5>(in, A, grid);
-    if (in->walkMinBlocks == 3) return launchWalk4K<CP, R, 3>(in, A, grid);
-    return launchWalk4K<CP, R, 4>(in, A, grid);
+    if (preOrder) return launchWalk4K<CP, R, true>(in, A, grid);
+    return launchWalk4K<CP, R, false>(in, A, grid);
 }
 
 template <int CP>

@@ -31,24 +31,23 @@ namespace b200 {
 
 namespace {
 
-// TIP = 0: a compact-tip child goes through the same contraction with a one-hot x (no memory traffic, no extra code path);
-// TIP = 1: its value is column s of the stored P matrix (one 32-B load per pattern, no arithmetic) -- the LSU / FP64
-//          trade-off is measured, not guessed (B200_TIP_MODE)
-//          TIP = 2: the columns of P for the five possible tip symbols (4 states + gap) of all categories are staged once per
-//          (op, child) in a per-warp shared-memory table by a handful of lanes; every pattern then picks its 32-B column
-//          with two LDS.128 -- no FP64 work, no dependent global load (the default)
+// Compact-tip children: at CP <= 8 (TABLE) the columns of P for the five possible tip symbols (4 states + gap) of all
+// categories are staged once per (op, child) in a per-warp shared-memory table by a handful of lanes; every pattern then
+// picks its 32-B column with two LDS.128 -- no FP64 work, no dependent global load.  At CP = 16 and 32 a tip goes through
+// the same contraction as an internal child, with a one-hot x (no memory traffic, no extra code path).
 __device__ __forceinline__ double absBits(double v) {       // |v| on the integer pipe (the FP64 pipe is the busy one here)
     return __hiloint2double(__double2hiint(v) & 0x7fffffff, __double2loint(v));
 }
 
-template <typename T, int CP, int R, bool ALIGNED, bool FIRST, int TIP>
+template <typename T, int CP, int R, bool ALIGNED, bool FIRST>
 __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)[16], int child, int matIdx, bool fromRegisters,
                                            int cc, size_t off0, int p0, bool catValid, int pBegin, int pEnd, double (&d)[R][4],
                                            double* tab) {
     constexpr int G = 32 / CP;
+    constexpr bool TABLE = CP <= 8;
     const int S = A.S;
     const bool tip = child < 0;
-    if (TIP == 2 && tip) {
+    if (TABLE && tip) {
         const int lane = threadIdx.x & 31;
         const uint8_t* t = A.states + (size_t)(-child - 1) * A.Ppad;
         int s[R];
@@ -80,24 +79,6 @@ __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)
             const double2 lo = col[0], hi = col[1];
             if (FIRST) { d[r][0] = lo.x; d[r][1] = lo.y; d[r][2] = hi.x; d[r][3] = hi.y; }
             else { d[r][0] *= lo.x; d[r][1] *= lo.y; d[r][2] *= hi.x; d[r][3] *= hi.y; }
-        }
-        return;
-    }
-    if (TIP == 1 && tip) {
-        const uint8_t* t = A.states + (size_t)(-child - 1) * A.Ppad;
-        const double* m = A.mats + (size_t)matIdx * A.matStride + cc * 4;
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const int p = p0 + r * G;
-            const int s = (ALIGNED || (catValid && p >= pBegin && p < pEnd)) ? (int)__ldg(t + p) : S;
-            double v[4];
-            if (s < S) ldg256_ro(m + 4 * CP * s, v);
-            else {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) v[i] = (i < S) ? 1.0 : 0.0;
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) d[r][i] = FIRST ? v[i] : d[r][i] * v[i];
         }
         return;
     }
@@ -138,9 +119,10 @@ __device__ __forceinline__ void childTermE(const WalkArgs& A, const double (&Vi)
     }
 }
 
-template <typename T, int CP, int R, bool ALIGNED, int TIP>
+template <typename T, int CP, int R, bool ALIGNED>
 __device__ __forceinline__ void walk4eBody(const WalkArgs& A) {
     constexpr int G = 32 / CP;
+    constexpr bool TABLE = CP <= 8;
     const int lane = threadIdx.x & 31;
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int c = lane / G;
@@ -151,10 +133,10 @@ __device__ __forceinline__ void walk4eBody(const WalkArgs& A) {
     const int cc = catValid ? c : 0;
     const size_t off0 = ((size_t)cc * A.Ppad + p0) * 4;
     const int last = range.y - 1;
-    // per-warp tip tables (TIP == 2): [child slot][CP][5][4] doubles
-    __shared__ __align__(16) double tipTab[TIP == 2 ? 4 * 2 * CP * 20 : 2];
-    double* tab1 = tipTab + (TIP == 2 ? ((threadIdx.x >> 5) * 2) * CP * 20 : 0);
-    double* tab2 = tab1 + (TIP == 2 ? CP * 20 : 0);
+    // per-warp tip tables: [child slot][CP][5][4] doubles
+    __shared__ __align__(16) double tipTab[TABLE ? 4 * 2 * CP * 20 : 2];
+    double* tab1 = tipTab + (TABLE ? ((threadIdx.x >> 5) * 2) * CP * 20 : 0);
+    double* tab2 = tab1 + (TABLE ? CP * 20 : 0);
 
     // V^-1 in vector registers (the tip selects and the first contraction read it), V stays in the constant bank: both in
     // uniform registers do not fit (64 > 63) and ptxas would spill.  The asm keeps ptxas from folding the copy back.
@@ -187,12 +169,12 @@ __device__ __forceinline__ void walk4eBody(const WalkArgs& A) {
         if (lane < 2) {
             const int mi = lane == 0 ? cur.pfM1 : cur.pfM2;
             if (mi >= 0) prefetchL1(A.evecs + (size_t)mi * CP * 4);            // all categories of a branch: one 128-B line
-        } else if (TIP != 0 && lane >= 8 && lane < 16) {
+        } else if (TABLE && lane >= 8 && lane < 16) {
             const int mi = lane < 12 ? cur.pfM1 : cur.pfM2;                     // matrix rows, should a child be a compact tip
             if (mi >= 0) prefetchL1(A.mats + (size_t)mi * A.matStride + (lane & 3) * 4 * CP);
         }
-        childTermE<T, CP, R, ALIGNED, true, TIP>(A, Vi, cur.c1, cur.m1, (cur.pad_ & 2) != 0, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab1);
-        childTermE<T, CP, R, ALIGNED, false, TIP>(A, Vi, cur.c2, cur.m2, false, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab2);
+        childTermE<T, CP, R, ALIGNED, true>(A, Vi, cur.c1, cur.m1, (cur.pad_ & 2) != 0, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab1);
+        childTermE<T, CP, R, ALIGNED, false>(A, Vi, cur.c2, cur.m2, false, cc, off0, p0, catValid, cur.pBegin, cur.pEnd, d, tab2);
         if (R != 1) nxt = loadOp(A.ops + min(k + 1, last));
         T* dg = static_cast<T*>(A.partials) + (size_t)cur.dest * A.stride + off0;
 #pragma unroll
@@ -223,21 +205,21 @@ __device__ __forceinline__ void walk4eBody(const WalkArgs& A) {
     }
 }
 
-template <int CP, int R, bool ALIGNED, int MINB, int TIP>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R, bool ALIGNED>
+__global__ void __launch_bounds__(128, 4)
 k_walk4e(const WalkArgs A) {
-    walk4eBody<double, CP, R, ALIGNED, TIP>(A);
+    walk4eBody<double, CP, R, ALIGNED>(A);
 }
 
 // fp32 partials storage (PRECISION_SINGLE)
-template <int CP, int R, bool ALIGNED, int MINB, int TIP>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R, bool ALIGNED>
+__global__ void __launch_bounds__(128, 4)
 k_walk4es(const WalkArgs A) {
-    walk4eBody<float, CP, R, ALIGNED, TIP>(A);
+    walk4eBody<float, CP, R, ALIGNED>(A);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// k_walk4p -- the same arithmetic with PER-WARP ASYNCHRONOUS OPERAND STAGING (the default for aligned lists, CP <= 8).
+// k_walk4p -- the same arithmetic with PER-WARP ASYNCHRONOUS OPERAND STAGING (every aligned list at CP <= 8).
 //
 // What bounds k_walk4e with the matrices gone: no pipe near its peak, but "long scoreboard" stalls on first uses of
 // small per-op operands -- the op record, the tips' state bytes, the
@@ -296,10 +278,13 @@ __device__ __forceinline__ void sts256(double2* p, const double (&v)[4]) {
 
 // dynamic shared memory of a 4-warp block's sibling stack: [slot][warp][R][2][32] 16-byte entries
 constexpr size_t stackBytes(int slots, int R) { return (size_t)slots * 4 * R * 64 * sizeof(double2); }
-// the instances that carry the sibling stack: CP = 4 at the default launch bound of 3 blocks, R <= 4.  ptxas keeps them
-// without a spill and the stack keeps their 3 blocks per SM; elsewhere (other CP, launch bounds 4-6, R = 8) the slot code
-// would cost spills or blocks, so those instances are built without it and ignore the slot bytes
-__host__ __device__ constexpr bool stackBuilt(int CP, int R, int MINB) { return CP == 4 && MINB == 3 && R <= 4; }
+// the instances that carry the sibling stack: CP = 4, launched at 3 blocks per SM.  ptxas keeps them without a spill and
+// the stack keeps their 3 blocks per SM; at other category counts the slot code would cost spills or blocks, so those
+// instances are built without it and ignore the slot bytes
+__host__ __device__ constexpr bool stackBuilt(int CP) { return CP == 4; }
+// launch bound of k_walk4p / k_walk4ps: 3 blocks let ptxas keep CP = 4 without a spill and 4 blocks still fit -- the
+// fastest setting where it was swept (BASELINE.md 6.7)
+constexpr int stagedMinBlocks(int CP) { return CP == 4 ? 3 : 4; }
 
 template <int CP, int R, bool VIRT>
 struct WarpStage {
@@ -516,38 +501,39 @@ __device__ __forceinline__ void walk4pBody(const WalkArgs& A) {
     }
 }
 
-template <int CP, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R>
+__global__ void __launch_bounds__(128, stagedMinBlocks(CP))
 k_walk4p(const WalkArgs A) {
-    walk4pBody<double, CP, R, false, stackBuilt(CP, R, MINB)>(A);
+    walk4pBody<double, CP, R, false, stackBuilt(CP)>(A);
 }
 
-template <int CP, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R>
+__global__ void __launch_bounds__(128, stagedMinBlocks(CP))
 k_walk4ps(const WalkArgs A) {
-    walk4pBody<float, CP, R, false, stackBuilt(CP, R, MINB)>(A);
+    walk4pBody<float, CP, R, false, stackBuilt(CP)>(A);
 }
 
-// lists that read virtual cherries: twice the tip tables per warp stage
-template <int CP, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
+// lists that read virtual cherries: twice the tip tables per warp stage.  One launch bound: with 3 blocks ptxas keeps the
+// doubled staging of k_walk4pv in registers without a spill at every CP and R
+template <int CP, int R>
+__global__ void __launch_bounds__(128, 3)
 k_walk4pv(const WalkArgs A) {
-    walk4pBody<double, CP, R, true, stackBuilt(CP, R, MINB)>(A);
+    walk4pBody<double, CP, R, true, stackBuilt(CP)>(A);
 }
 
-template <int CP, int R, int MINB>
-__global__ void __launch_bounds__(128, MINB)
+template <int CP, int R>
+__global__ void __launch_bounds__(128, 3)
 k_walk4pvs(const WalkArgs A) {
-    walk4pBody<float, CP, R, true, stackBuilt(CP, R, MINB)>(A);
+    walk4pBody<float, CP, R, true, stackBuilt(CP)>(A);
 }
 
 // stackSlots: the sibling stack of the phase (dynamic shared memory; 0 on instances built without it).  The kernel's
 // limit is set once per device to the deepest stack it can get (kStackSlots slots), never lowered: instances on other host
 // threads launch the same kernel with other depths.  No carveout preference: the driver sizes shared memory per launch, so
 // launches without a stack keep the larger L1.
-template <auto KERNEL, int CP, int R, int MINB>
+template <auto KERNEL, int CP, int R>
 cudaError_t launchStaged(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
-    const size_t smem = stackBuilt(CP, R, MINB) ? stackBytes(stackSlots, R) : 0;
+    const size_t smem = stackBuilt(CP) ? stackBytes(stackSlots, R) : 0;
     if (smem > 0) {
         static std::atomic<unsigned long long> limitSet{0};             // one bit per device
         const unsigned long long bit = 1ull << (in->device & 63);
@@ -568,18 +554,14 @@ cudaError_t launchStaged(Instance* in, const WalkArgs& A, dim3 grid, int stackSl
     return cudaGetLastError();
 }
 
-template <typename T, int CP, int R, int MINB>
-cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
-    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4ps<CP, R, MINB>, CP, R, MINB>(in, A, grid, stackSlots);
-    else return launchStaged<k_walk4p<CP, R, MINB>, CP, R, MINB>(in, A, grid, stackSlots);
-}
-
-// one launch bound only (B200_WALK_MINB does not apply): with 3 blocks ptxas keeps the doubled staging in registers without
-// a spill at every R the virtual kernel serves (R = 8 phases keep their cherries, see walk4pServes)
 template <typename T, int CP, int R>
-cudaError_t launchPV(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots) {
-    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4pvs<CP, R, 3>, CP, R, 3>(in, A, grid, stackSlots);
-    else return launchStaged<k_walk4pv<CP, R, 3>, CP, R, 3>(in, A, grid, stackSlots);
+cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots, bool virt) {
+    if (virt) {
+        if constexpr (sizeof(T) == 4) return launchStaged<k_walk4pvs<CP, R>, CP, R>(in, A, grid, stackSlots);
+        else return launchStaged<k_walk4pv<CP, R>, CP, R>(in, A, grid, stackSlots);
+    }
+    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4ps<CP, R>, CP, R>(in, A, grid, stackSlots);
+    else return launchStaged<k_walk4p<CP, R>, CP, R>(in, A, grid, stackSlots);
 }
 
 // recipe rows [buffer][2][16 * CP] of the virtual cherries a list produces: items (buffer, m1, m2, -)
@@ -625,74 +607,44 @@ __global__ void k_cherry_store_f32(const int4* items, int count, float* partials
     cherryStoreBody(items, count, partials, stride, states, recipes, S, C, CP, Ppad);
 }
 
-template <typename T, int CP, int R, bool ALIGNED, int MINB, int TIP>
+template <typename T, int CP, int R, bool ALIGNED>
 cudaError_t launchK(Instance* in, const WalkArgs& A, dim3 grid) {
-    if constexpr (sizeof(T) == 4) k_walk4es<CP, R, ALIGNED, MINB, TIP><<<grid, 128, 0, in->stream>>>(A);
-    else k_walk4e<CP, R, ALIGNED, MINB, TIP><<<grid, 128, 0, in->stream>>>(A);
+    if constexpr (sizeof(T) == 4) k_walk4es<CP, R, ALIGNED><<<grid, 128, 0, in->stream>>>(A);
+    else k_walk4e<CP, R, ALIGNED><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
-// shipped configuration per category count: R in {1, 4} x {aligned, windows}, tips through the shared-memory column table
-// (CP <= 8) or the contraction; CP = 4 (the Gamma-4 workloads the metric is quoted on) additionally carries the tuning space
-// behind B200_WALK_R / B200_WALK_MINB / B200_TIP_MODE
 // patterns per thread of a phase: a thin phase (few walks in flight) is latency-bound, one pattern group per thread gives
-// the most warps per op
+// the most warps per op; R = 2 is built for CP = 4 only
 int phaseR(const Instance* in, int nSubs, int maxWindow) {
     const int G = 32 / in->matCP;
     const long walks = (long)nSubs * ((maxWindow + G * in->walkR - 1) / (G * in->walkR));
     if ((in->thinR1 && walks < (long)in->smCount * 8) || in->walkR == 1) return 1;
-    if (in->matCP == 4 && (in->walkR == 8 || in->walkR == 2)) return in->walkR;
+    if (in->matCP == 4 && in->walkR == 2) return 2;
     return 4;
 }
 
 bool stagedWalk(const Instance* in, int R, bool aligned) {
     const int G = 32 / in->matCP;
     // predicate-free only when a warp's G*R patterns can never straddle the end of the padded pattern axis
-    return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4 && (R == 1 ? in->thinTipMode : in->tipMode) == 3;
+    return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4;
 }
 
 // stackSlots: slots per warp of the phase's sibling stack (0 = none)
 template <typename T, int CP, int R>
 cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt, int stackSlots) {
     constexpr int G = 32 / CP;
-    constexpr int TIPD = CP <= 8 ? 2 : 0;
     const int warps = (maxWindow + G * R - 1) / (G * R);
     dim3 grid((warps + 3) / 4, nSubs);
     if constexpr (CP <= 8 && G * R >= 4) {
-        if (stagedWalk(in, R, aligned)) {                          // per-warp asynchronous operand staging (k_walk4p)
-            if (virt) {
-                if constexpr (R == 8) return cudaErrorInvalidValue;
-                else return launchPV<T, CP, R>(in, A, grid, stackSlots);
-            }
-            if constexpr (CP == 4) {
-                // a launch bound of 3 blocks lets ptxas keep its registers without a spill and 4 blocks still fit -- the
-                // fastest setting where it was swept, unless B200_WALK_MINB says otherwise
-                const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;
-                if (minb >= 6) return launchP<T, CP, R, 6>(in, A, grid, stackSlots);
-                if (minb == 5) return launchP<T, CP, R, 5>(in, A, grid, stackSlots);
-                if (minb == 3) return launchP<T, CP, R, 3>(in, A, grid, stackSlots);
-            }
-            return launchP<T, CP, R, 4>(in, A, grid, stackSlots);
-        }
+        // per-warp asynchronous operand staging (k_walk4p): every aligned list at CP <= 8, since G * R >= 4 there
+        if (stagedWalk(in, R, aligned)) return launchP<T, CP, R>(in, A, grid, stackSlots, virt);
     }
     if (virt) return cudaErrorInvalidValue;                        // only k_walk4p reads virtual cherries
-    if (!aligned || in->Ppad % (G * R) != 0) return launchK<T, CP, R, false, 4, TIPD>(in, A, grid);
-    if constexpr (CP == 4 && R >= 2) {
-        const int minb = in->walkMinBlocks, tip = in->tipMode;
-        if (tip == 0) {
-            if (minb >= 5) return launchK<T, CP, R, true, 5, 0>(in, A, grid);
-            if (minb == 3) return launchK<T, CP, R, true, 3, 0>(in, A, grid);
-            return launchK<T, CP, R, true, 4, 0>(in, A, grid);
-        }
-        if (tip == 1) {
-            if (minb >= 5) return launchK<T, CP, R, true, 5, 1>(in, A, grid);
-            return launchK<T, CP, R, true, 4, 1>(in, A, grid);
-        }
-        if (minb >= 6) return launchK<T, CP, R, true, 6, 2>(in, A, grid);
-        if (minb == 5) return launchK<T, CP, R, true, 5, 2>(in, A, grid);
-        if (minb == 3) return launchK<T, CP, R, true, 3, 2>(in, A, grid);
+    if constexpr (CP > 8) {
+        if (aligned && in->Ppad % (G * R) == 0) return launchK<T, CP, R, true>(in, A, grid);
     }
-    return launchK<T, CP, R, true, 4, TIPD>(in, A, grid);
+    return launchK<T, CP, R, false>(in, A, grid);
 }
 
 template <typename T, int CP>
@@ -700,7 +652,6 @@ cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool a
     const int R = phaseR(in, nSubs, maxWindow);
     if (R == 1) return launchR<T, CP, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     if constexpr (CP == 4) {
-        if (R == 8) return launchR<T, CP, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         if (R == 2) return launchR<T, CP, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     }
     return launchR<T, CP, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
@@ -708,15 +659,11 @@ cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool a
 
 }  // namespace
 
-bool walkStackBuilt(const Instance* in) {
-    const int minb = in->walkMinBlocksSet ? in->walkMinBlocks : 3;     // the launch bound launchR picks for k_walk4p
-    return stackBuilt(in->matCP, in->walkR == 8 ? 8 : 4, minb);
-}
+bool walkStackBuilt(const Instance* in) { return stackBuilt(in->matCP); }
 
 bool walk4pServes(const Instance* in, int nSubs, int maxWindow) {
     if (in->matCP == 0) return false;
-    const int R = phaseR(in, nSubs, maxWindow);
-    return R != 8 && stagedWalk(in, R, true);        // R = 8 (B200_WALK_R=8): the virtual kernel would spill
+    return stagedWalk(in, phaseR(in, nSubs, maxWindow), true);
 }
 
 // eigen: [V (16, row-major Evec[i][k]) | V^-1 (16, Ievc[k][j])], padded to 4 x 4 with zeros
@@ -743,13 +690,11 @@ cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int n
         }
     }
     switch (in->matCP) {
-#ifndef B200_W4E_QUICK
         case 1: return launchCP<double, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         case 2: return launchCP<double, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         case 8: return launchCP<double, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         case 16: return launchCP<double, 16>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
         case 32: return launchCP<double, 32>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-#endif
         default: return launchCP<double, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
     }
 }

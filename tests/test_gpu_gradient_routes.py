@@ -233,7 +233,7 @@ R_ENV = {1: {}, 2: {"B200_WALK_R": "2", "B200_THIN_R1": "0"}, 4: {"B200_WALK_R":
 @pytest.mark.parametrize("R", [1, 2, 4])
 @pytest.mark.parametrize("C", CATS)
 def test_preorder4_every_cp_and_r(C, R, P):
-    """Route: 4-state pre-order walk k_walk4<CP, R, 4, true> (kernels.cu launchWalk4 -> launchWalk4T<CP>), CP =
+    """Route: 4-state pre-order walk k_walk4<CP, R, true> (kernels.cu launchWalk4 -> launchWalk4T<CP>), CP =
     matCP = C rounded up to a power of two (beagleCreateInstance); C = 40 has matCP = 0 and takes k_walk_generic
     (launchWalkGeneric, Sp = 4).  R = 1: the default rule of beagleCreateInstance halves walkR while a subtree has fewer
     warps than SMs, and launchWalk4T's thin rule (walks < smCount * 8) picks R = 1 anyway.  R = 2 / 4: B200_WALK_R
@@ -252,7 +252,7 @@ def test_preorder4_every_cp_and_r(C, R, P):
 
 @pytest.mark.parametrize("C,tips,P", [(4, 200, 5000), (24, 64, 2000)])
 def test_preorder4_natural_r4(C, tips, P):
-    """Route: k_walk4<CP, 4, 4, true> by the default rules alone: walkR stays 4 in beagleCreateInstance because
+    """Route: k_walk4<CP, 4, true> by the default rules alone: walkR stays 4 in beagleCreateInstance because
     Ppad / (32/CP * 4) >= smCount (1250 warps at CP = 4, 500 at CP = 32), and the phases of planPreorderPhases are wide
     enough that launchWalk4T's thin rule (walks < smCount * 8) does not apply."""
     tw = Twin(4, C, tips, P, seed=7 + C, partialTips=0.1)
@@ -288,7 +288,7 @@ def _pre_scaling(tw, phase):
 @pytest.mark.parametrize("S,C", [(4, 4), (20, 2), (70, 1)])
 def test_scaled_preorder_list(S, C, log):
     """Route: pre-order ops with destinationScaleWrite / destinationScaleRead (factors a previous list wrote) and a
-    cumulative index, on the 4-state walk (k_walk4<4, R, 4, true>, matCP = 4), the DMMA walk
+    cumulative index, on the 4-state walk (k_walk4<4, R, true>, matCP = 4), the DMMA walk
     (k_walk_mma<3, .., PRE = true>: Sp = 24, launchWalkGeneric with genericMma) and the FMA generic walk (k_walk_generic:
     Sp = 72 has no DMMA instance).  The walk rescales by the per-pattern maximum and stores the factor (log under
     SCALERS_LOG); accumulateInList adds the written factors' logs to the cumulative buffer after the phases.  Partials,

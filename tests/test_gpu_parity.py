@@ -12,6 +12,7 @@ import pytest
 import helpers as H
 from beast_mcmc_b200 import beagle
 from harness import evomodel as em, treedatalikelihood as tdl
+from test_gpu_virtual_cherries import NONE, Case, _with_env
 
 pytestmark = pytest.mark.gpu
 
@@ -182,10 +183,10 @@ def test_mcmc_reenactment_store_restore():
 
 def test_walk_variants_agree():
     """Matrix-form FMA walk: planned order == caller order, bitwise (same arithmetic).  The eigen-form walk (the default:
-    P x evaluated as V (e * (V^-1 x)), walk4e.cu) in its tuning variants agrees with it to rounding."""
+    P x evaluated as V (e * (V^-1 x)), walk4e.cu) in its orders and tilings agrees with it to rounding."""
     import os
     tree, pats, model, site = H.synthetic_case(120, 700, 4, seed=4)
-    keys = ("B200_REORDER", "B200_EIGEN_WALK", "B200_WALK_R", "B200_TIP_MODE", "B200_WALK_MINB")
+    keys = ("B200_REORDER", "B200_EIGEN_WALK", "B200_WALK_R")
 
     def run(**env):
         for k, v in env.items():
@@ -201,15 +202,44 @@ def test_walk_variants_agree():
 
     vals = [run(B200_EIGEN_WALK="0", B200_REORDER=r) for r in ("0", "1")]
     assert all(v == vals[0] for v in vals), vals
-    # eigen form: asynchronous operand staging (default, TIP_MODE 3) in several tilings; shared-memory tip table (2), tip
-    # column from global (1), tips through the contraction (0)
-    eigen = [run(), run(B200_REORDER="0"), run(B200_WALK_R="2"), run(B200_WALK_R="8"), run(B200_WALK_MINB="5"),
-             run(B200_WALK_MINB="3"), run(B200_TIP_MODE="2"), run(B200_TIP_MODE="2", B200_WALK_R="1"),
-             run(B200_TIP_MODE="1"), run(B200_TIP_MODE="1", B200_WALK_MINB="5"),
-             run(B200_TIP_MODE="0"), run(B200_TIP_MODE="0", B200_WALK_R="8")]
+    # eigen form: asynchronous operand staging (k_walk4p) in both op orders and several tilings
+    eigen = [run(), run(B200_REORDER="0"), run(B200_WALK_R="2"), run(B200_WALK_R="1")]
     assert all(_rel(v, vals[0]) <= 1e-13 for v in eigen), (eigen, vals[0])
-    # same arithmetic whatever the tiling or the way a tip's P column reaches the thread: bit-identical
-    assert len(set(eigen[:10])) == 1, eigen
+    # same arithmetic whatever the order or the tiling: bit-identical
+    assert len(set(eigen)) == 1, eigen
+
+
+@pytest.mark.parametrize("R", [1, 2, 4])
+def test_window_walk_bit_equal_to_staged_walk(R, capfd):
+    """At CP <= 8 an aligned list runs on the staged walk k_walk4p, a list with pattern windows (by partition) on
+    k_walk4e<CP, R, false>, whose compact tips pick their P column from a per-warp shared-memory table.  Both take the
+    same products in the same order: one partition over every pattern gives the internal partials of the plain list bit for
+    bit.  CP = 4; B200_WALK_R and B200_THIN_R1=0 fix the tiling R of every phase."""
+    case = Case(T=64, P=1000, C=4, seed=17)
+    env = {"B200_WALK_R": str(R), "B200_THIN_R1": "0", "B200_BEAGLE_DEBUG": "1"}
+
+    def run(by_partition):
+        inst = case.create(True)
+        if by_partition:
+            inst.setPatternPartitions(1, np.zeros(case.P, dtype=np.int32))
+        case.matrices(inst, [n for n in range(case.N) if n != case.root])
+        if by_partition:
+            flat = []
+            for n, a, b in case.ops:
+                flat += [n, NONE, NONE, a, case.mat(a), b, case.mat(b), 0, NONE]
+            inst.updatePartialsByPartition(np.array(flat, dtype=np.int32), len(case.ops))
+        else:
+            case.update(inst, case.ops)
+        out = [case.partials(inst, n) for n, _, _ in case.ops]
+        inst.finalize()
+        return out
+
+    staged = _with_env(env, lambda: run(False))
+    assert "staged walk" in capfd.readouterr().err
+    window = _with_env(env, lambda: run(True))
+    assert "staged walk" not in capfd.readouterr().err
+    for (n, _, _), a, b in zip(case.ops, staged, window):
+        assert np.array_equal(a, b), n
 
 
 def test_by_partition_equals_separate_instances():

@@ -95,7 +95,7 @@ def sass_excerpts():
             for op in pat.findall(line):
                 key = re.sub(r"\.(CONSTANT|STRONG|GPU|SYS).*", "", op)
                 per[name][key] = per[name].get(key, 0) + 1
-    keep = ("k_walk4p<4, 4, 3>", "k_walk4ps<4, 4, 3>", "k_walk4p<4, 1, 3>", "k_walk4pv<4, 4, 3>", "k_walk4pv<4, 1, 3>", "k_walk4e<4, 4, true, 4, 2>", "k_walk4<4, 4, 4, false>", "k_walk_mma<8, 4, false, false, 2>",
+    keep = ("k_walk4p<4, 4>", "k_walk4ps<4, 4>", "k_walk4p<4, 1>", "k_walk4pv<4, 4>", "k_walk4pv<4, 1>", "k_walk4e<4, 4, false>", "k_walk4<4, 4, false>", "k_walk_mma<8, 4, false, false, 2>",
             "k_walk_mma<8, 4, false, false, 1>", "k_walk_mma<3, 4, false, true, 2>", "k_transition_mma<8>", "k_incremental<4>", "k_root", "k_exchange_sum", "k_cross_mma<8>",
             "k_edge_derivatives_mma<8>")
     with open(os.path.join(P, f"{R}_sass_excerpts.txt"), "w") as f:

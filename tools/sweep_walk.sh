@@ -1,14 +1,14 @@
 #!/bin/bash
 # Kernel-variant sweep for the 4-state walk (run on the GPU box): one bench line per setting.
-# columns: reorder minBlocks phaseT(0=auto) R(patterns/thread) Tmin oversub
+# columns: reorder phaseT(0=auto) R(patterns/thread) Tmin oversub
 mkdir -p gpurun_out
 python bench.py --steps 5 --warmup 3 --no-cpu-baseline > /dev/null 2>&1   # builds the alignment cache
-CFGS=${CFGS:-"1 5 0 2 4 3;1 5 0 2 4 2;1 5 0 2 8 2;1 4 0 4 4 2;1 5 0 2 16 2;1 5 0 2 4 1"}
+CFGS=${CFGS:-"1 0 2 4 3;1 0 2 4 2;1 0 2 8 2;1 0 4 4 2;1 0 2 16 2;1 0 2 4 1"}
 IFS=';' read -ra LIST <<< "$CFGS"
 for cfg in "${LIST[@]}"; do
   set -- $cfg
-  echo "reorder=$1 minb=$2 phaseT=$3 R=$4 Tmin=$5 oversub=$6"
-  B200_REORDER=$1 B200_WALK_MINB=$2 B200_PHASE_T=$3 B200_WALK_R=$4 B200_PHASE_TMIN=$5 B200_PHASE_OVERSUB=$6 \
+  echo "reorder=$1 phaseT=$2 R=$3 Tmin=$4 oversub=$5"
+  B200_REORDER=$1 B200_PHASE_T=$2 B200_WALK_R=$3 B200_PHASE_TMIN=$4 B200_PHASE_OVERSUB=$5 \
     python bench.py --steps ${STEPS:-100} --warmup 5 --no-cpu-baseline $BENCH_ARGS 2>&1 | python -c "
 import sys, json
 for l in sys.stdin:
