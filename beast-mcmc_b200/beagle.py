@@ -169,6 +169,9 @@ _SIGNATURES = {
     "b200DebugAncestralRows": ([_IP, _IP, _IP, _I, _I, _I], _I),
     "b200SampleMarkovJumps": ([_I, _IP, _IP, _IP, _DP, _I, _I, _I, _I, _I, _I, _DP, _I, C.c_ulonglong, C.c_ulonglong, _IP, _IP,
                                _DP, _DP], _I),
+    "b200SampleSubstitutionHistories": ([_I, _IP, _IP, _IP, _DP, _I, _I, _I, _I, _I, _DP, _DP, _I, C.c_ulonglong,
+                                         C.c_ulonglong, _IP, _IP, _DP, _DP, _IP, C.c_longlong, C.POINTER(C.c_longlong), _DP,
+                                         _IP], _I),
     "b200GetSourceHash": ([], C.c_char_p),
     "b200GetFusedLaunches": ([_I], _L),
     "b200RootLogLikelihoodsByPartitionDevice": ([_I, _IP, _IP, _IP, _IP, _IP, _I, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)], _I),
@@ -501,6 +504,48 @@ class BeagleJNIImpl(Beagle):
                                                     categoryRatesIndex, regs[1], G, seed, drawIndex, ptr(outs[0], _IP),
                                                     ptr(outs[1], _IP), ptr(outs[2], _DP), ptr(outs[3], _DP)))
         return outs
+
+    def sampleSubstitutionHistories(self, nodeBuffers, parentRows, matrixIndices, edgeLengths, rootBuffer,
+                                    categoryWeightsIndex, stateFrequenciesIndex, categoryRatesIndex, rateMatrix,
+                                    registerMatrices, seed, drawIndex, states=True, categories=True, branchCounts=True,
+                                    patternCounts=True, jumpCounts=True, events=True):
+        """Complete substitution histories by uniformization, conditioned on one joint ancestral draw
+        (b200SampleSubstitutionHistories): rows and edgeLengths as in sampleMarkovJumps, rateMatrix [S][S] the generator Q,
+        registerMatrices [registers][S][S] -> (states int32 [rows][patternCount], categories int32 [patternCount],
+        branchCounts [registers][rows], patternCounts [registers][patternCount], jumpCounts int32 [rows][patternCount],
+        eventTimes [events], eventStates int32 [events]); the events are in (row, pattern, time) order.  An output switched
+        off by its flag is None and not copied back; with events, a sizing call first gives the arrays their length."""
+        nb, pr, mi = _ip(nodeBuffers), _ip(parentRows), _ip(matrixIndices)
+        count = len(nb[0])
+        assert len(pr[0]) == count and len(mi[0]) == count
+        lengths = _dp(np.asarray(edgeLengths, dtype=np.float64).reshape(count))
+        Q = _dp(np.asarray(rateMatrix, dtype=np.float64).reshape(-1))
+        regs = np.ascontiguousarray(registerMatrices, dtype=np.float64)
+        G = regs.shape[0] if regs.ndim == 3 else 1
+        regs = _dp(regs.reshape(-1))
+        P = self.patternCount
+        ptr = lambda a, t: None if a is None else a.ctypes.data_as(t)
+
+        def call(outs, capacity, total, times, states_):
+            return self._lib.b200SampleSubstitutionHistories(
+                self.instance, nb[1], pr[1], mi[1], lengths[1], count, rootBuffer, categoryWeightsIndex,
+                stateFrequenciesIndex, categoryRatesIndex, Q[1], regs[1], G, seed, drawIndex, ptr(outs[0], _IP),
+                ptr(outs[1], _IP), ptr(outs[2], _DP), ptr(outs[3], _DP), ptr(outs[4], _IP), capacity, total,
+                ptr(times, _DP), ptr(states_, _IP))
+
+        total = C.c_longlong(0)
+        times = eventStates = None
+        if events:
+            self._check("sampleSubstitutionHistories", call((None,) * 5, 0, C.byref(total), None, None))
+            times, eventStates = np.zeros(total.value), np.zeros(total.value, dtype=np.int32)
+        outs = (np.zeros((count, P), dtype=np.int32) if states else None,
+                np.zeros(P, dtype=np.int32) if categories else None,
+                np.zeros((G, count)) if branchCounts else None,
+                np.zeros((G, P)) if patternCounts else None,
+                np.zeros((count, P), dtype=np.int32) if jumpCounts else None)
+        self._check("sampleSubstitutionHistories",
+                    call(outs, total.value, C.byref(total) if events else None, times, eventStates))
+        return outs + (times, eventStates)
 
 
 class BeagleFactory:

@@ -20,6 +20,11 @@
 // same sample and look up, per drawn branch pair (i -> j), the conditional expectation N_g,c,r[i][j] of every register g
 // that k_jump_conditional wrote beforehand.  Pattern totals stay in registers; per-(row, pattern) values go to a
 // [g][row][P] workspace that k_jump_branch_totals reduces in a fixed order.
+//
+// Substitution histories (b200SampleSubstitutionHistories, DESIGN.md §7.3): the sampler (Jumps = false) leaves the end
+// states in the scratch; k_unif_powers tabulates the powers of the uniformized chain R = I + Q/μ, and k_histories draws one
+// complete history per (row >= 1, pattern) by uniformization, once for the registers and jump counts and, after an
+// exclusive scan of the counts (k_scan_tiles, k_scan_tile_sums), once more to write the events at their offsets.
 #include "walk4.cuh"
 
 #include <algorithm>
@@ -46,6 +51,18 @@ __host__ __device__ __forceinline__ uint64_t philox4x64_10(uint64_t k0, uint64_t
         c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
     }
     return c0;
+}
+
+// all four words of the same block, in place of the counter (the histories' uniforms; the sampler keeps the function above)
+__host__ __device__ __forceinline__ void philox4x64_10_words(uint64_t k0, uint64_t k1, uint64_t& c0, uint64_t& c1, uint64_t& c2,
+                                                             uint64_t& c3) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r > 0) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
+        const uint64_t lo0 = 0xD2E7470EE14C6C93ull * c0, hi0 = mulhi64(0xD2E7470EE14C6C93ull, c0);
+        const uint64_t lo1 = 0xCA5A826395121157ull * c2, hi1 = mulhi64(0xCA5A826395121157ull, c2);
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+    }
 }
 
 __device__ __forceinline__ double uniformAt(const AncestralArgs& a, int p, int row) {
@@ -344,6 +361,217 @@ k_jump_branch_totals(const MarkovJumpArgs m, int count, int P) {
     if (threadIdx.x == 0) m.branch[(size_t)g * count + r] = red[0];
 }
 
+// ---- substitution histories by uniformization (b200SampleSubstitutionHistories, DESIGN.md §7.3) ------------------------------
+__host__ __device__ constexpr size_t powersSmemDoubles(int S) { return (size_t)S * S + 2 * (size_t)S; }
+
+// (R^n)[i][b] for n = 0..N at powers[b][n][i]: one block per end state b, v_n = R v_{n-1} from v_0 = e_b, R in shared memory
+__global__ void __launch_bounds__(256)
+k_unif_powers(const double* R, double* powers, int S, int N) {
+    extern __shared__ double sm[];
+    double* Rs = sm;
+    double* v = Rs + (size_t)S * S;                         // [2][S], ping-pong
+    const int b = blockIdx.x;
+    for (int idx = threadIdx.x; idx < S * S; idx += blockDim.x) Rs[idx] = R[idx];
+    for (int i = threadIdx.x; i < S; i += blockDim.x) v[i] = i == b ? 1.0 : 0.0;
+    __syncthreads();
+    double* out = powers + (size_t)b * (N + 1) * S;
+    for (int n = 0;; ++n) {
+        const double* cur = v + (n & 1) * S;
+        double* nxt = v + ((n + 1) & 1) * S;
+        for (int i = threadIdx.x; i < S; i += blockDim.x) out[(size_t)n * S + i] = cur[i];
+        if (n == N) break;
+        for (int i = threadIdx.x; i < S; i += blockDim.x) {
+            double acc = 0.0;
+            for (int j = 0; j < S; ++j) acc += Rs[i * S + j] * cur[j];
+            nxt[i] = acc;
+        }
+        __syncthreads();
+    }
+}
+
+// uniform j of one (row, pattern) pair: word j mod 4 of the Philox block at counter (drawIndex, global pattern, row,
+// 1 + j / 4).  The last block is kept, so ascending j costs one block per four uniforms.
+struct PairUniforms {
+    uint64_t seed, c0, c1, c2;
+    uint64_t w0, w1, w2, w3;
+    long long block;
+    __device__ PairUniforms(uint64_t s, uint64_t d, uint64_t p, uint64_t r) : seed(s), c0(d), c1(p), c2(r), block(-1) {}
+    __device__ __forceinline__ double operator()(int j) {
+        const long long blk = j >> 2;
+        if (blk != block) {
+            w0 = c0; w1 = c1; w2 = c2; w3 = 1 + (uint64_t)blk;
+            philox4x64_10_words(seed, 0, w0, w1, w2, w3);
+            block = blk;
+        }
+        const int k = j & 3;
+        const uint64_t x = k == 0 ? w0 : k == 1 ? w1 : k == 2 ? w2 : w3;
+        return (double)(x >> 11) * 0x1.0p-53;
+    }
+};
+
+// One complete history of the branch above row r >= 1 for pattern p, per thread.  Events = false: the register values of
+// every (row, pattern) to perRow and its event count to jumps; Events = true: the same history again, its events written
+// at the scanned offsets.
+template <bool Events>
+__global__ void __launch_bounds__(128)
+k_histories(const HistoryArgs h) {
+    const size_t t = (size_t)blockIdx.x * 128 + threadIdx.x;
+    if (t >= (size_t)(h.count - 1) * h.P) return;
+    const int r = 1 + (int)(t / h.P), p = (int)(t % h.P);
+    const size_t cell = (size_t)r * h.P + p;
+    const int S = h.S, N = h.N;
+    const int a = h.states[(size_t)__ldg(h.rows + r).y * h.P + p], b = h.states[cell];
+    const double len = h.lengths[r];
+    const double tau = len * h.rates[h.categories[p]];
+    const double x = h.mu * tau;
+    const double* col = h.powers + (size_t)b * (N + 1) * S;  // (R^n)[i][b] at col[n S + i]
+    PairUniforms u(h.seed, h.drawIndex, (uint64_t)(h.pOffset + p), (uint64_t)r);    // j = 0 .. n - 1
+    PairUniforms v(h.seed, h.drawIndex, (uint64_t)(h.pOffset + p), (uint64_t)r);    // j = n .. 2n - 1
+    // 1. the number of uniformized jumps, ∝ π_n (R^n)[a][b]; once π_n underflows to 0 every later weight is 0 too
+    const double pi0 = exp(-x);
+    double total = 0.0, pi = pi0;
+    for (int k = 0; k <= N && pi > 0.0; ++k) {
+        total += pi * col[(size_t)k * S + a];
+        pi = pi * x / (k + 1);
+    }
+    const double target = u(0) * total;
+    int n = -1, lastPos = 0;
+    double cum = 0.0;
+    pi = pi0;
+    for (int k = 0; k <= N && pi > 0.0; ++k) {
+        const double w = pi * col[(size_t)k * S + a];
+        cum += w;
+        if (w > 0.0) lastPos = k;
+        if (target < cum) { n = k; break; }
+        pi = pi * x / (k + 1);
+    }
+    if (n < 0) n = lastPos;                                 // 0 when every weight is 0: the pair is impossible, no events
+    // 2.-4. intermediate states, ascending jump times, registers
+    double reg[Events ? 1 : kMaxJumpRegisters] = {};
+    long long out = 0;
+    if constexpr (Events) out = h.tileOffsets[cell / kScanTile] + h.localOffsets[cell];
+    int s = a, events = 0;
+    double U = 0.0;
+    for (int k = 1; k <= n; ++k) {
+        int next = b;
+        if (k < n) {
+            const double* Rs = h.R + (size_t)s * S;
+            const double* tail = col + (size_t)(n - k) * S;
+            double tot = 0.0;
+            for (int j = 0; j < S; ++j) tot += Rs[j] * tail[j];
+            const double tt = u(k) * tot;
+            int last = 0;
+            double run = 0.0;
+            next = -1;
+            for (int j = 0; j < S; ++j) {
+                const double w = Rs[j] * tail[j];
+                run += w;
+                if (w > 0.0) last = j;
+                if (tt < run) { next = j; break; }
+            }
+            if (next < 0) next = last;
+        }
+        // U_k = 1 - (1 - U_{k-1}) v^{1/(n-k+1)}, written with expm1 so that small steps keep their relative accuracy
+        const double Uk = U - (1.0 - U) * expm1(log(v(n + k - 1)) / (n - k + 1));
+        if constexpr (!Events) {
+#pragma unroll
+            for (int g = 0; g < kMaxJumpRegisters; ++g) {
+                if (g >= h.G) break;
+                reg[g] += h.registers[((size_t)g * S + s) * S + s] * tau * (Uk - U);
+            }
+        }
+        if (next != s) {
+            if constexpr (Events) {
+                if (h.eventTimes != nullptr) h.eventTimes[out] = len * Uk;
+                if (h.eventStates != nullptr) h.eventStates[out] = next;
+                ++out;
+            } else {
+                const double q = h.Q[(size_t)s * S + next];
+#pragma unroll
+                for (int g = 0; g < kMaxJumpRegisters; ++g) {
+                    if (g >= h.G) break;
+                    reg[g] += h.registers[((size_t)g * S + s) * S + next] / q;
+                }
+                ++events;
+            }
+        }
+        s = next;
+        U = Uk;
+    }
+    if constexpr (!Events) {
+        if (h.perRow != nullptr) {
+#pragma unroll
+            for (int g = 0; g < kMaxJumpRegisters; ++g) {
+                if (g >= h.G) break;
+                h.perRow[((size_t)g * h.count + r) * h.P + p] = reg[g] + h.registers[((size_t)g * S + s) * S + s] * tau * (1.0 - U);
+            }
+        }
+        if (h.jumps != nullptr) h.jumps[cell] = events;
+    }
+}
+
+// pattern totals Σ_{r >= 1} n_g[r][p], added in row order: one thread per (g, p)
+__global__ void __launch_bounds__(256)
+k_history_pattern_totals(const double* perRow, double* pattern, int G, int count, int P) {
+    const size_t t = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (t >= (size_t)G * P) return;
+    const size_t g = t / P, p = t % P;
+    double s = 0.0;
+    for (int r = 1; r < count; ++r) s += perRow[(g * count + r) * P + p];
+    pattern[t] = s;
+}
+
+// exclusive scan of n ints, first pass: tile-local offsets (256 threads x 8 items per tile) and each tile's sum
+__global__ void __launch_bounds__(256)
+k_scan_tiles(const int* in, size_t n, int* local, long long* tileSums) {
+    __shared__ int part[256];
+    const int tid = threadIdx.x;
+    const size_t base = (size_t)blockIdx.x * kScanTile + (size_t)tid * 8;
+    int x[8], s = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { x[i] = base + i < n ? in[base + i] : 0; s += x[i]; }
+    part[tid] = s;
+    __syncthreads();
+    for (int o = 1; o < 256; o <<= 1) {
+        const int y = tid >= o ? part[tid - o] : 0;
+        __syncthreads();
+        part[tid] += y;
+        __syncthreads();
+    }
+    int run = part[tid] - s;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        if (base + i < n) local[base + i] = run;
+        run += x[i];
+    }
+    if (tid == 255) tileSums[blockIdx.x] = part[255];
+}
+
+// second pass, one block: the tile sums become exclusive tile offsets in place, and tileSums[tiles] the total
+__global__ void __launch_bounds__(1024)
+k_scan_tile_sums(long long* tileSums, int tiles) {
+    __shared__ long long part[1024];
+    const int tid = threadIdx.x, per = (tiles + 1023) / 1024;
+    const int lo = min(tiles, tid * per), hi = min(tiles, lo + per);
+    long long s = 0;
+    for (int i = lo; i < hi; ++i) s += tileSums[i];
+    part[tid] = s;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+        const long long y = tid >= o ? part[tid - o] : 0;
+        __syncthreads();
+        part[tid] += y;
+        __syncthreads();
+    }
+    long long run = part[tid] - s;
+    for (int i = lo; i < hi; ++i) {
+        const long long v = tileSums[i];
+        tileSums[i] = run;
+        run += v;
+    }
+    if (tid == 1023) tileSums[tiles] = part[1023];
+}
+
 }  // namespace
 
 bool markovJumpsFit(const Instance* in) {
@@ -373,6 +601,47 @@ cudaError_t launchMarkovJumps(Instance* in, const AncestralArgs& a, const Markov
         k_ancestral_warp<true><<<(a.P + 3) / 4, 128, 0, in->stream>>>(a, m);
     }
     if (m.branch != nullptr) k_jump_branch_totals<<<dim3(a.count, m.G), 256, 0, in->stream>>>(m, a.count, a.P);
+    return cudaGetLastError();
+}
+
+bool historiesFit(const Instance* in) {
+    return powersSmemDoubles(in->S) * sizeof(double) <= std::max<size_t>(in->maxSmemOptin, 48 << 10);
+}
+
+cudaError_t launchHistories(Instance* in, const HistoryArgs& h, double* branch, double* pattern, long long* tileSums) {
+    const int S = h.S;
+    const size_t smem = powersSmemDoubles(S) * sizeof(double);
+    if (smem > (48 << 10)) {
+        // the device's whole opt-in, never a smaller value: instances on other host threads launch the same kernel
+        const cudaError_t e = cudaFuncSetAttribute(k_unif_powers, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)in->maxSmemOptin);
+        if (e != cudaSuccess) return e;
+    }
+    k_unif_powers<<<S, std::min(256, (S + 31) / 32 * 32), smem, in->stream>>>(h.R, const_cast<double*>(h.powers), S, h.N);
+    const size_t pairs = (size_t)(h.count - 1) * h.P;
+    if (pairs > 0) k_histories<false><<<(unsigned)((pairs + 127) / 128), 128, 0, in->stream>>>(h);
+    if (branch != nullptr) {
+        MarkovJumpArgs m{};
+        m.perRow = h.perRow;
+        m.branch = branch;
+        m.patternWeights = in->dPatternWeights;
+        k_jump_branch_totals<<<dim3(h.count, h.G), 256, 0, in->stream>>>(m, h.count, h.P);
+    }
+    if (pattern != nullptr)
+        k_history_pattern_totals<<<(unsigned)(((size_t)h.G * h.P + 255) / 256), 256, 0, in->stream>>>(h.perRow, pattern, h.G,
+                                                                                                        h.count, h.P);
+    if (tileSums != nullptr) {
+        const size_t n = (size_t)h.count * h.P;
+        const int tiles = (int)((n + kScanTile - 1) / kScanTile);
+        k_scan_tiles<<<tiles, 256, 0, in->stream>>>(h.jumps, n, h.localOffsets, tileSums);
+        k_scan_tile_sums<<<1, 1024, 0, in->stream>>>(tileSums, tiles);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launchHistoryEvents(Instance* in, const HistoryArgs& h) {
+    const size_t pairs = (size_t)(h.count - 1) * h.P;
+    if (pairs > 0) k_histories<true><<<(unsigned)((pairs + 127) / 128), 128, 0, in->stream>>>(h);
     return cudaGetLastError();
 }
 

@@ -170,7 +170,7 @@ void destroyInstance(Instance* in) {
     if (in->hMapped) cudaFreeHost(in->hMapped); cudaFree(in->dRates); cudaFree(in->dWeights);
     cudaFree(in->dFreqs); cudaFree(in->dScale); cudaFree(in->dPatternWeights);
     cudaFree(in->dPatternPartitions); cudaFree(in->dSite); cudaFree(in->dBlockSums); cudaFree(in->dOut);
-    cudaFree(in->dCounter); cudaFree(in->dStage); cudaFree(in->dScratch);
+    cudaFree(in->dCounter); cudaFree(in->dStage); cudaFree(in->dScratch); cudaFree(in->dEvents);
     if (in->hStage) cudaFreeHost(in->hStage);
     if (in->hOut) cudaFreeHost(in->hOut);
     for (int c = 0; c < T_CLASSES; ++c)
@@ -2397,6 +2397,25 @@ int b200SampleMarkovJumps(int instance, const int* nodeBuffers, const int* paren
                              registerCount, seed, drawIndex, 0, outStates, outCategories, outBranchCounts, outPatternCounts);
 }
 
+int b200SampleSubstitutionHistories(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                    const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                                    int stateFrequenciesIndex, int categoryRatesIndex, const double* rateMatrix,
+                                    const double* registerMatrices, int registerCount, unsigned long long seed,
+                                    unsigned long long drawIndex, int* outStates, int* outCategories, double* outBranchCounts,
+                                    double* outPatternCounts, int* outJumpCounts, long long eventCapacity,
+                                    long long* outEventCount, double* outEventTimes, int* outEventStates) {
+    SH(instance, shSampleSubstitutionHistories(sh, nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer,
+                                               categoryWeightsIndex, stateFrequenciesIndex, categoryRatesIndex, rateMatrix,
+                                               registerMatrices, registerCount, seed, drawIndex, outStates, outCategories,
+                                               outBranchCounts, outPatternCounts, outJumpCounts, eventCapacity, outEventCount,
+                                               outEventTimes, outEventStates));
+    return sampleSubstitutionHistories(instance, nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer,
+                                       categoryWeightsIndex, stateFrequenciesIndex, categoryRatesIndex, rateMatrix,
+                                       registerMatrices, registerCount, seed, drawIndex, 0, outStates, outCategories,
+                                       outBranchCounts, outPatternCounts, outJumpCounts, eventCapacity, outEventCount,
+                                       outEventTimes, outEventStates);
+}
+
 }  // extern "C"
 
 // the sampler's argument rules and the written state of every buffer it reads: checked before anything is launched, the
@@ -2528,6 +2547,145 @@ int b200::sampleMarkovJumps(int instance, const int* nodeBuffers, const int* par
     if (outCategories != nullptr) memcpy(outCategories, ints.data(), sizeof(int) * P);
     if (outStates != nullptr) memcpy(outStates, ints.data() + P, sizeof(int) * R * P);
     return BEAGLE_SUCCESS;
+}
+
+int b200::checkHistoryArguments(int S, const double* rateMatrix, int registerCount, long long eventCapacity,
+                                const long long* outEventCount, const double* outEventTimes, const int* outEventStates,
+                                double* mu) {
+    if (rateMatrix == nullptr || registerCount < 1 || registerCount > kMaxJumpRegisters || eventCapacity < 0 ||
+        ((outEventTimes != nullptr || outEventStates != nullptr) && outEventCount == nullptr))
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    double m = 0.0;
+    for (int i = 0; i < S; ++i) {
+        for (int j = 0; j < S; ++j) {
+            const double q = rateMatrix[(size_t)i * S + j];
+            if (!std::isfinite(q) || (i != j && q < 0.0)) return BEAGLE_ERROR_OUT_OF_RANGE;
+        }
+        m = std::max(m, -rateMatrix[(size_t)i * S + i]);
+    }
+    for (int i = 0; i < S; ++i) {
+        double sum = 0.0;
+        for (int j = 0; j < S; ++j) sum += rateMatrix[(size_t)i * S + j];
+        if (std::fabs(sum) > 1e-9 * m) return BEAGLE_ERROR_OUT_OF_RANGE;
+    }
+    *mu = m;
+    return BEAGLE_SUCCESS;
+}
+
+int b200::sampleSubstitutionHistories(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                      const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                                      int stateFrequenciesIndex, int categoryRatesIndex, const double* rateMatrix,
+                                      const double* registerMatrices, int registerCount, unsigned long long seed,
+                                      unsigned long long drawIndex, int patternOffset, int* outStates, int* outCategories,
+                                      double* outBranchCounts, double* outPatternCounts, int* outJumpCounts,
+                                      long long eventCapacity, long long* outEventCount, double* outEventTimes,
+                                      int* outEventStates) {
+    GET_INSTANCE_LAZY(in, instance);
+    int rc = checkSampleRows(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex,
+                             stateFrequenciesIndex);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    double mu = 0.0;
+    rc = checkHistoryArguments(in->S, rateMatrix, registerCount, eventCapacity, outEventCount, outEventTimes, outEventStates,
+                               &mu);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    if (!validRange(categoryRatesIndex, in->nSets) || edgeLengths == nullptr || registerMatrices == nullptr)
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    double tauMax = 0.0;
+    for (int r = 1; r < count; ++r) {
+        if (!(std::isfinite(edgeLengths[r]) && edgeLengths[r] >= 0.0)) return BEAGLE_ERROR_OUT_OF_RANGE;
+        for (int c = 0; c < in->C; ++c) tauMax = std::max(tauMax, edgeLengths[r] * in->hRates[(size_t)categoryRatesIndex * in->C + c]);
+    }
+    const double xMax = mu * tauMax;
+    if (!(xMax <= 700.0) || !historiesFit(in)) return BEAGLE_ERROR_NO_IMPLEMENTATION;
+    const int N = (int)std::ceil(xMax + 12.0 * std::sqrt(xMax) + 12.0);
+    const bool wantEvents = outEventTimes != nullptr || outEventStates != nullptr;
+    const bool scan = wantEvents || outEventCount != nullptr;
+    const bool perRow = outBranchCounts != nullptr || outPatternCounts != nullptr;
+    const bool histories = perRow || outJumpCounts != nullptr || scan;
+    // scratch after the sampler's ints: Q | R [S][S], M [G][S][S], powers [S][N + 1][S], perRow [G][count][P], pattern
+    // [G][P], branch [G][count], then the ints jumps and tile-local offsets [count][P] and the tile offsets (as doubles)
+    const size_t G = registerCount, S = in->S, SS = S * S, R = count, P = in->P, RP = R * P;
+    const size_t tiles = (RP + kScanTile - 1) / kScanTile;
+    const size_t nPowers = S * (N + 1) * S, nPerRow = perRow ? G * RP : 0;
+    const size_t intDoubles = (RP + 1) / 2;
+    const size_t extra = histories ? 2 * SS + G * SS + nPowers + nPerRow + G * P + G * R + 2 * intDoubles + tiles + 1 : 0;
+    AncestralArgs a;
+    double* x = nullptr;
+    rc = prepareSample(in, nodeBuffers, parentRows, matrixIndices, count, rootBuffer, categoryWeightsIndex, stateFrequenciesIndex,
+                       seed, drawIndex, patternOffset, extra, a, &x);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    CUDA_OK(launchAncestral(in, a));
+    HistoryArgs h{};
+    double *dBranch = nullptr, *dPattern = nullptr;
+    long long* dTiles = nullptr;
+    if (histories) {
+        std::vector<double> Rm(SS);
+        for (size_t i = 0; i < S; ++i)
+            for (size_t j = 0; j < S; ++j)
+                Rm[i * S + j] = mu > 0.0 ? (i == j ? 1.0 : 0.0) + rateMatrix[i * S + j] / mu : (i == j ? 1.0 : 0.0);
+        double* dQ = x;
+        double* dR = dQ + SS;
+        double* dM = dR + SS;
+        double* dPowers = dM + G * SS;
+        h.perRow = perRow ? dPowers + nPowers : nullptr;
+        double* dPat = dPowers + nPowers + nPerRow;
+        double* dBr = dPat + G * P;
+        int* dJumps = reinterpret_cast<int*>(dBr + G * R);
+        h.localOffsets = reinterpret_cast<int*>(dBr + G * R + intDoubles);
+        dTiles = scan ? reinterpret_cast<long long*>(dBr + G * R + 2 * intDoubles) : nullptr;
+        dBranch = outBranchCounts != nullptr ? dBr : nullptr;
+        dPattern = outPatternCounts != nullptr ? dPat : nullptr;
+        rc = uploadSmall(in, dQ, rateMatrix, sizeof(double) * SS);
+        if (rc == BEAGLE_SUCCESS) rc = uploadSmall(in, dR, Rm.data(), sizeof(double) * SS);
+        if (rc == BEAGLE_SUCCESS) rc = uploadSmall(in, dM, registerMatrices, sizeof(double) * G * SS);
+        if (rc != BEAGLE_SUCCESS) return rc;
+        h.lengths = static_cast<const double*>(stage(in, edgeLengths, sizeof(double) * R));
+        if (h.lengths == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
+        h.G = registerCount; h.N = N; h.count = count; h.P = in->P; h.S = in->S; h.pOffset = patternOffset;
+        h.seed = seed; h.drawIndex = drawIndex; h.mu = mu;
+        h.rows = a.rows; h.states = a.outStates; h.categories = a.outCategories;
+        h.rates = in->dRates + (size_t)categoryRatesIndex * in->C;
+        h.Q = dQ; h.R = dR; h.powers = dPowers; h.registers = dM;
+        h.jumps = outJumpCounts != nullptr || scan ? dJumps : nullptr;
+        h.tileOffsets = dTiles;
+        if (h.jumps != nullptr) CUDA_OK(cudaMemsetAsync(h.jumps, 0, sizeof(int) * P, in->stream));     // row 0
+        CUDA_OK(launchHistories(in, h, dBranch, dPattern, dTiles));
+    }
+    // the fixed-size outputs come back in one round, with the event total when it is asked for
+    std::vector<int> ints(outStates != nullptr ? (size_t)(count + 1) * P : outCategories != nullptr ? P : 0);
+    if (!ints.empty())
+        CUDA_OK(cudaMemcpyAsync(ints.data(), a.outCategories, sizeof(int) * ints.size(), cudaMemcpyDeviceToHost, in->stream));
+    if (dBranch != nullptr)
+        CUDA_OK(cudaMemcpyAsync(outBranchCounts, dBranch, sizeof(double) * G * R, cudaMemcpyDeviceToHost, in->stream));
+    if (dPattern != nullptr)
+        CUDA_OK(cudaMemcpyAsync(outPatternCounts, dPattern, sizeof(double) * G * P, cudaMemcpyDeviceToHost, in->stream));
+    if (outJumpCounts != nullptr)
+        CUDA_OK(cudaMemcpyAsync(outJumpCounts, h.jumps, sizeof(int) * RP, cudaMemcpyDeviceToHost, in->stream));
+    long long total = 0;
+    if (scan) CUDA_OK(cudaMemcpyAsync(&total, dTiles + tiles, sizeof(long long), cudaMemcpyDeviceToHost, in->stream));
+    CUDA_OK(cudaStreamSynchronize(in->stream));
+    if (wantEvents && total <= eventCapacity && total > 0) {
+        const size_t bytes = (size_t)total * (sizeof(double) + sizeof(int));
+        if (bytes > in->eventBytes) {
+            cudaFree(in->dEvents);
+            in->dEvents = nullptr;
+            in->eventBytes = 0;
+            CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&in->dEvents), bytes));
+            in->eventBytes = bytes;
+        }
+        h.eventTimes = outEventTimes != nullptr ? reinterpret_cast<double*>(in->dEvents) : nullptr;
+        h.eventStates = outEventStates != nullptr ? reinterpret_cast<int*>(in->dEvents + sizeof(double) * total) : nullptr;
+        CUDA_OK(launchHistoryEvents(in, h));
+        if (h.eventTimes != nullptr)
+            CUDA_OK(cudaMemcpyAsync(outEventTimes, h.eventTimes, sizeof(double) * total, cudaMemcpyDeviceToHost, in->stream));
+        if (h.eventStates != nullptr)
+            CUDA_OK(cudaMemcpyAsync(outEventStates, h.eventStates, sizeof(int) * total, cudaMemcpyDeviceToHost, in->stream));
+        CUDA_OK(cudaStreamSynchronize(in->stream));
+    }
+    if (outCategories != nullptr) memcpy(outCategories, ints.data(), sizeof(int) * P);
+    if (outStates != nullptr) memcpy(outStates, ints.data() + P, sizeof(int) * RP);
+    if (outEventCount != nullptr) *outEventCount = total;
+    return wantEvents && total > eventCapacity ? BEAGLE_ERROR_OUT_OF_RANGE : BEAGLE_SUCCESS;
 }
 
 extern "C" {

@@ -208,6 +208,8 @@ struct Instance {
     bool debugLog = false;                    // B200_BEAGLE_DEBUG: per-launch diagnostics on stderr
     double* dScratch = nullptr;               // grow-only workspace of the derivative calls
     size_t scratchDoubles = 0;
+    char* dEvents = nullptr;                  // grow-only event arrays of b200SampleSubstitutionHistories
+    size_t eventBytes = 0;
     int partitionCount = 1;
     std::vector<int> partBegin, partEnd;      // contiguous pattern ranges per partition
     std::vector<int> hostPartitions;
@@ -358,5 +360,48 @@ int sampleMarkovJumps(int instance, const int* nodeBuffers, const int* parentRow
                       int eigenIndex, int categoryRatesIndex, const double* registerMatrices, int registerCount,
                       unsigned long long seed, unsigned long long drawIndex, int patternOffset, int* outStates,
                       int* outCategories, double* outBranchCounts, double* outPatternCounts);
+
+// ---- complete substitution histories by uniformization (ancestral.cu, DESIGN.md §7.3) -----------------------------------
+constexpr int kScanTile = 2048;           // items per tile of the jump-count scan
+struct HistoryArgs {
+    int G, N;                     // registers; the largest uniformized jump count of the call
+    int count, P, S;
+    int pOffset;                  // global index of pattern 0: the Philox counter carries it
+    unsigned long long seed, drawIndex;
+    double mu;                    // max_i -Q_ii (0 when Q = 0, and then R = I)
+    const int4* rows;             // the sampler's staged rows (parent row in .y)
+    const int* states;            // [count][P] drawn by the sampler
+    const int* categories;        // [P]
+    const double* rates;          // [C] of the chosen rate set
+    const double* lengths;        // [count] edge lengths (row 0 not read)
+    const double* Q;              // [S][S]
+    const double* R;              // [S][S] = I + Q / mu (I when mu = 0)
+    const double* powers;         // [S (b)][N + 1][S (i)]: (R^n)[i][b]
+    const double* registers;      // M [G][S][S]
+    double* perRow;               // [G][count][P] register value of every (row, pattern), or nullptr
+    int* jumps;                   // [count][P] event counts (row 0 written by the caller), or nullptr
+    int* localOffsets;            // [count][P] tile-local exclusive offsets of jumps
+    const long long* tileOffsets; // [tiles + 1] exclusive tile offsets, the total last
+    double* eventTimes;           // events pass: [total] or nullptr
+    int* eventStates;             // events pass: [total] or nullptr
+};
+// false when R and two state vectors do not fit in one block's shared memory (S above 169 on an H100)
+bool historiesFit(const Instance* in);
+// the power table, the first history pass, the requested totals (branch and pattern may be nullptr) and, when tileSums is
+// non-null, the exclusive scan of h.jumps
+cudaError_t launchHistories(Instance* in, const HistoryArgs& h, double* branch, double* pattern, long long* tileSums);
+// the second pass: the same histories, their events written at the scanned offsets
+cudaError_t launchHistoryEvents(Instance* in, const HistoryArgs& h);
+// api.cu: b200SampleSubstitutionHistories on one single-device instance; patternOffset as for sampleAncestralStates
+int sampleSubstitutionHistories(int instance, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                const double* edgeLengths, int count, int rootBuffer, int categoryWeightsIndex,
+                                int stateFrequenciesIndex, int categoryRatesIndex, const double* rateMatrix,
+                                const double* registerMatrices, int registerCount, unsigned long long seed,
+                                unsigned long long drawIndex, int patternOffset, int* outStates, int* outCategories,
+                                double* outBranchCounts, double* outPatternCounts, int* outJumpCounts, long long eventCapacity,
+                                long long* outEventCount, double* outEventTimes, int* outEventStates);
+// the argument checks of b200SampleSubstitutionHistories that need no instance state (also the sharded instance's)
+int checkHistoryArguments(int S, const double* rateMatrix, int registerCount, long long eventCapacity,
+                          const long long* outEventCount, const double* outEventTimes, const int* outEventStates, double* mu);
 
 }  // namespace b200

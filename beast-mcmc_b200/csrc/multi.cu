@@ -439,6 +439,90 @@ int shSampleMarkovJumps(Sharded* sh, const int* nodeBuffers, const int* parentRo
     return BEAGLE_SUCCESS;
 }
 
+// as shSampleMarkovJumps.  Round 1 gives every shard's fixed-size outputs, jump counts and event total; when events are
+// asked for and the total over all shards fits eventCapacity, round 2 draws each shard's events, and they are reassembled in
+// global (row, pattern) order from the shards' jump counts.
+int shSampleSubstitutionHistories(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                  const double* edgeLengths, int count, int rootBuffer, int wIdx, int fIdx, int rIdx,
+                                  const double* rateMatrix, const double* registerMatrices, int registerCount,
+                                  unsigned long long seed, unsigned long long drawIndex, int* outStates, int* outCategories,
+                                  double* outBranchCounts, double* outPatternCounts, int* outJumpCounts, long long eventCapacity,
+                                  long long* outEventCount, double* outEventTimes, int* outEventStates) {
+    double mu = 0.0;
+    if (count < 1) return BEAGLE_ERROR_OUT_OF_RANGE;
+    int rc = checkHistoryArguments(sh->S, rateMatrix, registerCount, eventCapacity, outEventCount, outEventTimes,
+                                   outEventStates, &mu);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    const bool wantEvents = outEventTimes != nullptr || outEventStates != nullptr;
+    const size_t G = registerCount;
+    std::vector<std::vector<int>> states(sh->g), cats(sh->g), jumps(sh->g), evStates(sh->g);
+    std::vector<std::vector<double>> branch(sh->g), pattern(sh->g), evTimes(sh->g);
+    std::vector<long long> events(sh->g, 0);
+    auto ptr = [](auto& v) { return v.empty() ? nullptr : v.data(); };
+    rc = sh->pool->run([&](int k) {
+        const size_t n = sh->count[k];
+        if (n == 0) return 0;
+        if (outStates != nullptr) states[k].resize((size_t)count * n);
+        if (outCategories != nullptr) cats[k].resize(n);
+        if (outBranchCounts != nullptr) branch[k].resize(G * count);
+        if (outPatternCounts != nullptr) pattern[k].resize(G * n);
+        if (outJumpCounts != nullptr || wantEvents) jumps[k].resize((size_t)count * n);
+        return sampleSubstitutionHistories(sh->child[k], nodeBuffers, parentRows, matrixIndices, edgeLengths, count, rootBuffer,
+                                           wIdx, fIdx, rIdx, rateMatrix, registerMatrices, registerCount, seed, drawIndex,
+                                           sh->begin[k], ptr(states[k]), ptr(cats[k]), ptr(branch[k]), ptr(pattern[k]),
+                                           ptr(jumps[k]), 0, outEventCount != nullptr ? &events[k] : nullptr, nullptr, nullptr);
+    });
+    if (rc != 0) return rc;
+    long long total = 0;
+    for (int k = 0; k < sh->g; ++k) total += events[k];
+    const bool fits = total <= eventCapacity;
+    if (wantEvents && fits && total > 0) {
+        rc = sh->pool->run([&](int k) {
+            if (sh->count[k] == 0 || events[k] == 0) return 0;
+            if (outEventTimes != nullptr) evTimes[k].resize(events[k]);
+            if (outEventStates != nullptr) evStates[k].resize(events[k]);
+            long long got = 0;
+            return sampleSubstitutionHistories(sh->child[k], nodeBuffers, parentRows, matrixIndices, edgeLengths, count,
+                                               rootBuffer, wIdx, fIdx, rIdx, rateMatrix, registerMatrices, registerCount, seed,
+                                               drawIndex, sh->begin[k], nullptr, nullptr, nullptr, nullptr, nullptr, events[k],
+                                               &got, ptr(evTimes[k]), ptr(evStates[k]));
+        });
+        if (rc != 0) return rc;
+        std::vector<long long> pos(sh->g, 0);                    // next event of each shard
+        long long out = 0;
+        for (int r = 0; r < count; ++r)
+            for (int k = 0; k < sh->g; ++k) {
+                const size_t n = sh->count[k];
+                long long m = 0;
+                for (size_t p = 0; p < n; ++p) m += jumps[k][(size_t)r * n + p];
+                if (outEventTimes != nullptr)
+                    memcpy(outEventTimes + out, evTimes[k].data() + pos[k], sizeof(double) * m);
+                if (outEventStates != nullptr)
+                    memcpy(outEventStates + out, evStates[k].data() + pos[k], sizeof(int) * m);
+                pos[k] += m;
+                out += m;
+            }
+    }
+    if (outBranchCounts != nullptr) std::fill(outBranchCounts, outBranchCounts + G * count, 0.0);
+    for (int k = 0; k < sh->g; ++k) {
+        const size_t n = sh->count[k];
+        if (n == 0) continue;
+        if (outCategories != nullptr) memcpy(outCategories + sh->begin[k], cats[k].data(), sizeof(int) * n);
+        for (int r = 0; r < count; ++r) {
+            if (outStates != nullptr)
+                memcpy(outStates + (size_t)r * sh->P + sh->begin[k], states[k].data() + (size_t)r * n, sizeof(int) * n);
+            if (outJumpCounts != nullptr)
+                memcpy(outJumpCounts + (size_t)r * sh->P + sh->begin[k], jumps[k].data() + (size_t)r * n, sizeof(int) * n);
+        }
+        if (outBranchCounts != nullptr) for (size_t q = 0; q < G * count; ++q) outBranchCounts[q] += branch[k][q];
+        if (outPatternCounts != nullptr)
+            for (size_t g = 0; g < G; ++g)
+                memcpy(outPatternCounts + g * sh->P + sh->begin[k], pattern[k].data() + g * n, sizeof(double) * n);
+    }
+    if (outEventCount != nullptr) *outEventCount = total;
+    return wantEvents && !fits ? BEAGLE_ERROR_OUT_OF_RANGE : BEAGLE_SUCCESS;
+}
+
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq) {
     if (outSumSq != nullptr) return BEAGLE_ERROR_NO_IMPLEMENTATION;

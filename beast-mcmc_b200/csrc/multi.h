@@ -21,6 +21,12 @@ int shSampleMarkovJumps(Sharded* sh, const int* nodeBuffers, const int* parentRo
                         const double* edgeLengths, int count, int rootBuffer, int wIdx, int fIdx, int eigenIndex, int rIdx,
                         const double* registerMatrices, int registerCount, unsigned long long seed, unsigned long long drawIndex,
                         int* outStates, int* outCategories, double* outBranchCounts, double* outPatternCounts);
+int shSampleSubstitutionHistories(Sharded* sh, const int* nodeBuffers, const int* parentRows, const int* matrixIndices,
+                                  const double* edgeLengths, int count, int rootBuffer, int wIdx, int fIdx, int rIdx,
+                                  const double* rateMatrix, const double* registerMatrices, int registerCount,
+                                  unsigned long long seed, unsigned long long drawIndex, int* outStates, int* outCategories,
+                                  double* outBranchCounts, double* outPatternCounts, int* outJumpCounts, long long eventCapacity,
+                                  long long* outEventCount, double* outEventTimes, int* outEventStates);
 int shCrossProducts(Sharded* sh, const int* post, const int* pre, const int* rIdx, const int* wIdx, const double* lengths,
                     int count, double* outSum, double* outSumSq);
 }  // namespace b200

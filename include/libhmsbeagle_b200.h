@@ -426,6 +426,54 @@ BEAGLE_DLLEXPORT int b200SampleMarkovJumps(int instance, const int* nodeBuffers,
                                            const double* registerMatrices, int registerCount, unsigned long long seed,
                                            unsigned long long drawIndex, int* outStates, int* outCategories,
                                            double* outBranchCounts, double* outPatternCounts);
+/* Complete substitution histories on the device by uniformization, conditioned on ONE joint ancestral draw (what BEAST's
+ * Markov-jumps likelihood draws in Java with useUniformization / saveCompleteHistory; DESIGN.md section 7.3).  It needs only
+ * the generator, so non-reversible models with complex eigenvalues are served.
+ * Rows, seed and drawIndex exactly as in b200SampleAncestralStates: outStates and outCategories are bit-identical to what
+ * it returns (same Philox counters (drawIndex, global pattern, row, 0)).
+ *   rateMatrix [S][S] row-major, the generator Q (one per call, shared by all categories).  mu = max_i -Q_ii, R = I + Q/mu
+ *          (R = I and no events when mu = 0).  tau = r_c * edgeLengths[r] for row r >= 1, r_c the rate of the pattern's
+ *          drawn category c in set categoryRatesIndex.  N = ceil(mu tau_max + 12 sqrt(mu tau_max) + 12), tau_max the
+ *          largest tau over rows >= 1 and all categories; the powers R^n, n = 0..N, are formed on the device once per call.
+ *   Per (row r >= 1, pattern p) with parent state a and own state b:
+ *     1. n, the number of uniformized jumps, drawn with weights pi_n (R^n)[a][b], n = 0..N, pi_0 = exp(-mu tau),
+ *        pi_n = pi_{n-1} mu tau / n (the truncated distribution);
+ *     2. s_k for k = 1..n-1 drawn with weights R[s_{k-1}][j] (R^{n-k})[j][b] over j, s_0 = a, s_n = b;
+ *     3. U_0 = 0, U_k = 1 - (1 - U_{k-1}) v_k^{1/(n-k+1)} (computed as U_{k-1} - (1 - U_{k-1}) expm1(log(v_k)/(n-k+1)));
+ *     4. a jump with s_k = s_{k-1} is virtual and dropped; every other is an event (time edgeLengths[r] U_k from the
+ *        parent end, new state s_k).
+ *     Each draw is the sampler's inverse CDF (sequential fp64 sums; the first item whose sum exceeds u * total, else the
+ *     last of positive weight, else item 0).  When every weight of the n draw is 0 (b unreachable from a), n = 0.
+ *     Uniform j of the pair is word j mod 4 of the Philox4x64-10 block at counter (drawIndex, global pattern, r, 1 + j/4),
+ *     u = (x >> 11) 2^-53: j = 0 draws n, j = 1..n-1 the states, j = n..2n-1 are the v_k.
+ *   registerMatrices [registerCount][S][S] as in b200SampleMarkovJumps (counts M_ij = Q_ij R_ij off the diagonal, rewards
+ *          M = diag(r)).  n_g[r][p] = sum over events (i -> j) of M_g[i][j] / Q[i][j] + sum over segments k = 0..n of
+ *          M_g[s_k][s_k] tau (U_{k+1} - U_k), U_{n+1} = 1.  An event adds the register's weight of its change and time is in
+ *          tau units, so E[n_g | a, b] is the N_g[a][b] of b200SampleMarkovJumps.
+ * outBranchCounts[g * count + r] = sum_p w_p n_g[r][p] (row 0 is 0); outPatternCounts[g * patternCount + p] =
+ * sum_{r >= 1} n_g[r][p] in row order; outJumpCounts[r * patternCount + p] = the number of events (row 0 is 0).
+ * Events are stored in (row, pattern, time) order at the exclusive prefix sum of outJumpCounts: outEventTimes (edge-length
+ * units from the parent end) and outEventStates (the new state); *outEventCount receives their total.  Any output may be
+ * NULL; only what is asked for is computed past the sampler and copied back.  Both event arrays NULL is the sizing query.
+ * When events are asked for and their total exceeds eventCapacity, the event arrays are left untouched, *outEventCount and
+ * every fixed-size output are written, and the call returns BEAGLE_ERROR_OUT_OF_RANGE; the draw is a pure function of the
+ * arguments, so the call can be repeated with arrays of the right size.  No atomics: repeated calls are bit-identical.
+ * Every other error returns before anything is launched (deferred work included) and leaves every output untouched:
+ * BEAGLE_ERROR_OUT_OF_RANGE for whatever b200SampleAncestralStates rejects (its NULL-output rule aside), rateMatrix == NULL,
+ * an entry of it not finite, a negative off-diagonal entry or a row sum larger in magnitude than 1e-9 mu,
+ * categoryRatesIndex out of range, edgeLengths == NULL or an edgeLengths[r] (r >= 1) negative or not finite,
+ * registerMatrices == NULL, registerCount outside 1..8, eventCapacity < 0, an event array without outEventCount;
+ * BEAGLE_ERROR_NO_IMPLEMENTATION when mu tau_max > 700 (pi_0 would leave the normal range) or when S is so large that R and
+ * two state vectors do not fit in one block's shared memory (S above 169 on an H100). */
+BEAGLE_DLLEXPORT int b200SampleSubstitutionHistories(int instance, const int* nodeBuffers, const int* parentRows,
+                                                     const int* matrixIndices, const double* edgeLengths, int count,
+                                                     int rootBuffer, int categoryWeightsIndex, int stateFrequenciesIndex,
+                                                     int categoryRatesIndex, const double* rateMatrix,
+                                                     const double* registerMatrices, int registerCount,
+                                                     unsigned long long seed, unsigned long long drawIndex, int* outStates,
+                                                     int* outCategories, double* outBranchCounts, double* outPatternCounts,
+                                                     int* outJumpCounts, long long eventCapacity, long long* outEventCount,
+                                                     double* outEventTimes, int* outEventStates);
 /* Host-logic test hook (no CUDA): the row rules of b200SampleAncestralStates for an instance with bufferCount buffers and
  * matrixCount matrices; 0 or BEAGLE_ERROR_OUT_OF_RANGE. */
 BEAGLE_DLLEXPORT int b200DebugAncestralRows(const int* nodeBuffers, const int* parentRows, const int* matrixIndices, int count,
