@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 
 using namespace b200;
@@ -257,7 +258,7 @@ char gImplDesc[] = "sm_90a walk kernels: one launch per operation list, shared-m
 //   * inside a subtree ops run in Sethi-Ullman order (deeper-need child first), which minimises the
 //     number of live intermediate results;
 //   * every result is stored to global memory; inside a subtree walk the next op may take it from registers
-//     (forwardFromPrevious) and a later one from the sibling stack (assignStackSlots).
+//     (forwardOps4) and a later one from the sibling stack (assignStackSlots).
 // Lists with hazards the forest model does not cover (a buffer written twice, read-before-write,
 // a result consumed by two ops) run as ONE subtree in the caller's order.
 struct Sub { int begin, end, pBase, pLimit; };     // op positions [begin,end) applied to patterns [pBase,pLimit)
@@ -267,8 +268,20 @@ struct Plan {
     std::vector<int> phaseStart;     // index into subs; size = phases + 1
 };
 
-void planPhases(const std::vector<HostOp>& ops, int nBuffers, bool allowReorder, int fixedT, int wantSubs, int minT,
-                int smallRemainder, Plan& plan) {
+// what the planners take besides the list: the subtree bound (fixedT, or from the other three), whether a post-order list
+// may be reordered, and whether a pre-order list runs as phased subtree walks (else one launch per depth level)
+struct PlanParams {
+    int fixedT, wantSubs, minT, smallRemainder;
+    bool reorder, prePhases;
+    // per-phase subtree bound: enough subtrees to fill the machine, re-evaluated on what is left
+    // (a remainder of a couple of dozen ops is cheaper as one launch than as several tiny phases)
+    int bound(int remaining) const {
+        if (fixedT > 0) return fixedT;
+        return remaining <= smallRemainder ? remaining : std::max(minT, (remaining + wantSubs - 1) / wantSubs);
+    }
+};
+
+void planPhases(const std::vector<HostOp>& ops, int nBuffers, const PlanParams& pp, Plan& plan) {
     const int n = (int)ops.size();
     auto single = [&]() {
         plan.order.resize(n);
@@ -276,7 +289,7 @@ void planPhases(const std::vector<HostOp>& ops, int nBuffers, bool allowReorder,
         plan.subs.assign(1, Sub{0, n, 0, 0});
         plan.phaseStart = {0, 1};
     };
-    if (!allowReorder || n < 2) { single(); return; }
+    if (!pp.reorder || n < 2) { single(); return; }
     std::vector<int> writer(nBuffers, -1);
     for (int k = 0; k < n; ++k) {
         if (writer[ops[k].dest] >= 0) { single(); return; }
@@ -296,9 +309,7 @@ void planPhases(const std::vector<HostOp>& ops, int nBuffers, bool allowReorder,
     plan.subs.clear(); plan.phaseStart.assign(1, 0);
     int remaining = n;
     while (remaining > 0) {
-        // per-phase subtree bound: enough subtrees to fill the machine, re-evaluated on what is left
-        // (a remainder of a couple of dozen ops is cheaper as one launch than as several tiny phases)
-        const int T = fixedT > 0 ? fixedT : (remaining <= smallRemainder ? remaining : std::max(minT, (remaining + wantSubs - 1) / wantSubs));
+        const int T = pp.bound(remaining);
         for (int k = 0; k < n; ++k) {
             if (!alive[k]) continue;
             const int a = (ch0[k] >= 0 && alive[ch0[k]]) ? ch0[k] : -1;
@@ -373,8 +384,7 @@ void planLevels(const std::vector<HostOp>& ops, int nBuffers, Plan& plan) {
 // of extraction: the crown first, the many independent subtrees last.  Inside a subtree ops run in depth-first pre-order,
 // so the op after a node is its first child and finds pre[parent] in the walking thread's registers.
 // Anything the forest model does not cover (double write, read-before-write, a c2 produced in this list) -> planLevels.
-void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, int fixedT, int wantSubs, int minT,
-                        int smallRemainder, Plan& plan) {
+void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, const PlanParams& pp, Plan& plan) {
     const int n = (int)ops.size();
     std::vector<int> writer(nBuffers, -1), parent(n, -1);
     bool ok = n >= 2;
@@ -392,7 +402,7 @@ void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, int fixedT
     std::vector<std::vector<int>> phases;          // roots of the subtrees of each extracted phase
     int remaining = n;
     while (remaining > 0) {
-        const int T = fixedT > 0 ? fixedT : (remaining <= smallRemainder ? remaining : std::max(minT, (remaining + wantSubs - 1) / wantSubs));
+        const int T = pp.bound(remaining);
         for (int k = n - 1; k >= 0; --k) {          // children have larger indices than their parent
             if (!alive[k]) continue;
             size[k] = 1;
@@ -438,17 +448,45 @@ void planPreorderPhases(const std::vector<HostOp>& ops, int nBuffers, int fixedT
     }
 }
 
-// register forwarding: inside one subtree walk a thread re-reads, as a child, exactly the cell it wrote for the previous
-// op -- flag it (bit 1), with that child moved to position 1 (the product commutes exactly); tip: the op's virtual tips
-void forwardFromPrevious(Op4& d, const Op4& pv, bool preOrder, int4* tip) {
-    if (pv.pBegin != d.pBegin || pv.pEnd != d.pEnd) return;
-    const bool v1 = (d.pad_ & 4) != 0, v2 = (d.pad_ & 8) != 0;
-    if (d.c1 >= 0 && !v1 && d.c1 == pv.dest) d.pad_ |= 2;     // pre-order: pre[parent] is the previous result
-    else if (!preOrder && d.c2 >= 0 && !v2 && d.c2 == pv.dest) {
-        std::swap(d.c1, d.c2); std::swap(d.m1, d.m2);
-        if (tip) *tip = make_int4(tip->z, tip->w, tip->x, tip->y);
-        d.pad_ = (d.pad_ & ~12) | (v1 ? 8 : 0) | 2;
-    }
+// the planner of a non-empty list: by its kind (pre- or post-order) and the parameters
+void planList(const std::vector<HostOp>& ops, int nBuffers, const PlanParams& pp, Plan& plan) {
+    if (ops[0].kind != 1) planPhases(ops, nBuffers, pp, plan);
+    else if (pp.prePhases) planPreorderPhases(ops, nBuffers, pp, plan);
+    else planLevels(ops, nBuffers, plan);
+}
+
+// register forwarding over every subtree walk: a thread re-reads, as a child, exactly the cell it wrote for the previous
+// op -- flag it (bit 1), with that child moved to position 1 (the product commutes exactly).  A record's forwarding reads
+// only dest, pBegin and pEnd of the previous one, which forwarding never changes.  tips: the ops' virtual tips, or nullptr
+void forwardOps4(std::vector<Op4>& ops, const std::vector<Sub>& subs, bool preOrder, int4* tips) {
+    for (const Sub& s : subs)
+        for (int pos = s.begin + 1; pos < s.end; ++pos) {
+            Op4& d = ops[pos];
+            const Op4& pv = ops[pos - 1];
+            if (pv.pBegin != d.pBegin || pv.pEnd != d.pEnd) continue;
+            const bool v1 = (d.pad_ & 4) != 0, v2 = (d.pad_ & 8) != 0;
+            if (d.c1 >= 0 && !v1 && d.c1 == pv.dest) d.pad_ |= 2;     // pre-order: pre[parent] is the previous result
+            else if (!preOrder && d.c2 >= 0 && !v2 && d.c2 == pv.dest) {
+                std::swap(d.c1, d.c2); std::swap(d.m1, d.m2);
+                if (tips) tips[pos] = make_int4(tips[pos].z, tips[pos].w, tips[pos].x, tips[pos].y);
+                d.pad_ = (d.pad_ & ~12) | (v1 ? 8 : 0) | 2;
+            }
+        }
+}
+
+// the same on the tensor-pipe walk (one category, post-order lists): the warp that wrote the previous op's 16-pattern tile
+// still holds it in its accumulators -- flag the child (moved to position 1; the product commutes exactly)
+void forwardDevOps(std::vector<DevOp>& ops, const std::vector<Sub>& subs) {
+    for (const Sub& s : subs)
+        for (int pos = s.begin + 1; pos < s.end; ++pos) {
+            DevOp& d = ops[pos];
+            const DevOp& pv = ops[pos - 1];
+            if (pv.pBegin != d.pBegin || pv.pEnd != d.pEnd) continue;
+            if (d.c1 != nullptr && d.c1 == pv.dest) d.pad_ |= 2;
+            else if (d.c2 != nullptr && d.c2 == pv.dest) {
+                std::swap(d.c1, d.c2); std::swap(d.s1, d.s2); std::swap(d.m1, d.m2); d.pad_ |= 2;
+            }
+        }
 }
 
 // ---- sibling stack of the staged eigen walk (k_walk4p, walk4e.cu) -----------------------------------------------------
@@ -514,34 +552,38 @@ void assignStackSlots(std::vector<Op4>& ops, const std::vector<Sub>& subs, int d
     }
 }
 
-// launch the phases of a prepared plan (device-resident op records + subtree table)
-// eigenSlot >= 0: the 4-state list runs in eigen form (walk4e.cu) with that slot's V / V^-1; aligned: no pattern windows;
-// nSnap: virtual cherries the list produces (their recipes are snapshot first); virt: the records name virtual cherries;
-// phaseSlots: sibling-stack depth of each phase (eigen-form walks)
-cudaError_t launchPlan(Instance* in, const void* dOps, const void* dSubs, const std::vector<int>& phaseStart,
-                       const std::vector<int>& phaseSlots, bool fourPath, int maxWindow, bool preOrder, int eigenSlot = -1,
-                       bool aligned = false, const void* dSnap = nullptr, int nSnap = 0, const void* dVirtTips = nullptr) {
-    const bool virt = dVirtTips != nullptr;
+// kernel launches of a plan: the cherry snapshot, if any, and one per non-empty phase
+int launchCount(const PlanRecord& r) {
+    int launches = !r.cherries.empty();
+    for (size_t ph = 0; ph + 1 < r.phaseStart.size(); ++ph) launches += r.phaseStart[ph + 1] > r.phaseStart[ph];
+    return launches;
+}
+
+// launch the phases of a plan from its device block; eigenSlot >= 0: the 4-state list runs in eigen form (walk4e.cu) with
+// that slot's V / V^-1
+cudaError_t launchPlan(Instance* in, const PlanRecord& r, const void* dBlock, int eigenSlot) {
+    const char* block = static_cast<const char*>(dBlock);
+    const int4* dSubs = reinterpret_cast<const int4*>(block + r.subsOffset);
+    const int4* dVirtTips = r.readsVirtual ? reinterpret_cast<const int4*>(block + r.tipsOffset) : nullptr;
     cudaError_t e = cudaSuccess;
-    if (nSnap > 0) {
+    if (!r.cherries.empty()) {       // the recipes of the virtual cherries the list produces
         TimedScope ts(in, T_PARTIALS);
-        e = launchCherrySnapshot(in, static_cast<const int4*>(dSnap), nSnap);
+        e = launchCherrySnapshot(in, reinterpret_cast<const int4*>(block + r.snapOffset), (int)r.cherries.size());
     }
-    for (size_t ph = 0; ph + 1 < phaseStart.size() && e == cudaSuccess; ++ph) {
-        const int s0 = phaseStart[ph], s1 = phaseStart[ph + 1];
+    for (size_t ph = 0; ph + 1 < r.phaseStart.size() && e == cudaSuccess; ++ph) {
+        const int s0 = r.phaseStart[ph], s1 = r.phaseStart[ph + 1];
         if (s1 <= s0) continue;
         TimedScope ts(in, T_PARTIALS);
-        if (fourPath && eigenSlot >= 0 && !preOrder) {
-            e = launchWalk4E(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
-                             aligned, in->hEigen.data() + (size_t)eigenSlot * 36, static_cast<const int4*>(dVirtTips),
-                             ph < phaseSlots.size() ? phaseSlots[ph] : 0);
+        if (eigenSlot >= 0) {
+            e = launchWalk4E(in, static_cast<const Op4*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow, !r.byPartition,
+                             in->hEigen.data() + (size_t)eigenSlot * 36, dVirtTips,
+                             ph < r.phaseSlots.size() ? r.phaseSlots[ph] : 0);
             continue;
         }
-        if (virt) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
-        e = fourPath ? launchWalk4(in, static_cast<const Op4*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0, maxWindow,
-                                   preOrder)
-                     : launchWalkGeneric(in, static_cast<const DevOp*>(dOps), static_cast<const int4*>(dSubs) + s0, s1 - s0,
-                                         maxWindow, preOrder);
+        if (dVirtTips != nullptr) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
+        e = r.fourPath ? launchWalk4(in, static_cast<const Op4*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow, r.preOrder)
+                       : launchWalkGeneric(in, static_cast<const DevOp*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow,
+                                           r.preOrder);
     }
     return e;
 }
@@ -629,16 +671,14 @@ int prepareOps(Instance* in, const std::vector<HostOp>& hops, bool byPartition) 
         if (o.cum != BEAGLE_OP_NONE && !validRange(o.cum, in->nScale)) return BEAGLE_ERROR_OUT_OF_RANGE;
         if (byPartition && !validRange(o.part, in->partitionCount)) return BEAGLE_ERROR_OUT_OF_RANGE;
     }
-    {
-        // a child must hold data: compact states, partials, or the destination of an op of this very list
-        std::vector<char> written(in->nBuffers, 0);
-        for (const HostOp& o : hops) written[o.dest] = 1;
-        auto holdsData = [&](int b) { return written[b] || in->partials[b] != nullptr || in->states32[b] != nullptr; };
-        for (const HostOp& o : hops) {
-            if (!holdsData(o.c1) || !holdsData(o.c2)) return BEAGLE_ERROR_OUT_OF_RANGE;
-            // pre-order: c1 is pre[parent], a partials buffer by construction
-            if (o.kind == 1 && !written[o.c1] && in->states32[o.c1] != nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
-        }
+    // a child must hold data: compact states, partials, or the destination of an op of this very list
+    std::vector<char> written(in->nBuffers, 0);
+    for (const HostOp& o : hops) written[o.dest] = 1;
+    auto holdsData = [&](int b) { return written[b] || in->partials[b] != nullptr || in->states32[b] != nullptr; };
+    for (const HostOp& o : hops) {
+        if (!holdsData(o.c1) || !holdsData(o.c2)) return BEAGLE_ERROR_OUT_OF_RANGE;
+        // pre-order: c1 is pre[parent], a partials buffer by construction
+        if (o.kind == 1 && !written[o.c1] && in->states32[o.c1] != nullptr) return BEAGLE_ERROR_OUT_OF_RANGE;
     }
     for (const HostOp& o : hops) {
         if (ensurePartials(in, o.dest) == nullptr) return BEAGLE_ERROR_OUT_OF_MEMORY;
@@ -662,334 +702,134 @@ int eigenFormSlot(const Instance* in, const std::vector<HostOp>& hops) {
     return E;
 }
 
-int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartition) {
-    const int n = (int)hops.size();
-    if (n == 0) return BEAGLE_SUCCESS;
-    // ---- plan cache: MCMC re-issues identical lists all the time (every move that keeps the topology and
-    // dirties all nodes, in BEAST's two buffer-index parities); a hit skips validation, planning and the H2D copy.
-    static_assert(sizeof(HostOp) == 10 * sizeof(int), "HostOp is compared bytewise");
-    if (in->planCacheSize > 0) {
-        for (CachedPlan& cp : in->planCache) {
-            if (cp.dBlock == nullptr || cp.n != n || cp.byPartition != byPartition || cp.epoch != in->bufferEpoch ||
-                memcmp(cp.key.data(), hops.data(), sizeof(HostOp) * (size_t)n) != 0)
-                continue;
-            const int eigenSlot = cp.fourPath ? eigenFormSlot(in, hops) : -1;
-            // records that name virtual cherries need the eigen form, and an outside child read as a cherry must still be it
-            bool stale = cp.readsVirtual && eigenSlot < 0;
-            for (const CherryRef& x : cp.external)
-                stale = stale || (x.tip1 >= 0 && (in->cherryTip1[x.buf] != x.tip1 || in->cherryTip2[x.buf] != x.tip2));
-            if (stale) { cp.dropGraph(); cp.n = -1; continue; }
-            CUDA_OK(storeExternal(in, cp.external));
-            cp.lastUse = ++in->planClock;
-            cp.hits++;
-            const unsigned eigenGenNow = eigenSlot >= 0 ? in->eigenGen[eigenSlot] : 0u;
-            const void* dSnap = static_cast<char*>(cp.dBlock) + cp.snapOffset;
-            const int nSnap = (int)cp.cherries.size();
-            const void* dTips = cp.readsVirtual ? static_cast<char*>(cp.dBlock) + cp.tipsOffset : nullptr;
-            // a captured graph carries the kernel choice and V / V^-1 by value: stale once the eigen system moved on
-            if (cp.graphExec != nullptr && (cp.graphEigen != eigenSlot || cp.graphEigenGen != eigenGenNow)) {
-                // same kernels, new V / V^-1 (a substitution-model move): patch the captured launches in place
-                if (cp.graphAllEigen && eigenSlot >= 0 && cp.graphEigen == eigenSlot &&
-                    updateWalk4EGraph(cp.graphExec, cp.graphKernelNodes, in->hEigen.data() + (size_t)eigenSlot * 36) == cudaSuccess) {
-                    cp.graphEigenGen = eigenGenNow;
-                } else {
-                    cudaGetLastError();
-                    cp.dropGraph();
-                    cp.hits = 1;
-                    if (++cp.graphInvalidations >= 4) cp.graphFailed = true;     // the kernel choice flips every step: plain launches
-                }
-            }
-            // A plan that keeps coming back and needs several dependent launches is replayed as ONE graph launch:
-            // on small alignments the host-side launch cost, not the kernels, sets the pace.
-            int launches = nSnap > 0;
-            for (size_t ph = 0; ph + 1 < cp.phaseStart.size(); ++ph) launches += cp.phaseStart[ph + 1] > cp.phaseStart[ph];
-            // (in-list cumulative scaling stages its index lists per call: those plans keep the plain launches)
-            if (in->useGraphs && launches >= 2 && cp.cumGroups.empty()) {
-                if (cp.graphExec == nullptr && !cp.graphFailed && cp.hits >= 2 && !in->timing &&
-                    cudaStreamBeginCapture(in->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-                    const cudaError_t e1 = launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart,
-                                                      cp.phaseSlots, cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot,
-                                                      !cp.byPartition, dSnap, nSnap, dTips);
-                    cp.graphEigen = eigenSlot;
-                    cp.graphEigenGen = eigenGenNow;
-                    cudaGraph_t g = nullptr;
-                    const cudaError_t e2 = cudaStreamEndCapture(in->stream, &g);
-                    if (e1 != cudaSuccess || e2 != cudaSuccess || g == nullptr ||
-                        cudaGraphInstantiate(&cp.graphExec, g, 0) != cudaSuccess) {
-                        cp.graphExec = nullptr;
-                        cp.graphFailed = true;
-                        if (g) cudaGraphDestroy(g);
-                    } else {
-                        cp.graph = g;
-                        cp.graphKernelNodes.clear();
-                        cp.graphAllEigen = cp.fourPath && eigenSlot >= 0 && !cp.preOrder;
-                        size_t nn = 0;
-                        if (cudaGraphGetNodes(g, nullptr, &nn) == cudaSuccess && nn > 0) {
-                            std::vector<cudaGraphNode_t> nodes(nn);
-                            cudaGraphNodeType ty;
-                            if (cudaGraphGetNodes(g, nodes.data(), &nn) == cudaSuccess)
-                                for (size_t q = 0; q < nn; ++q)
-                                    if (cudaGraphNodeGetType(nodes[q], &ty) == cudaSuccess && ty == cudaGraphNodeTypeKernel)
-                                        cp.graphKernelNodes.push_back(nodes[q]);
-                        }
-                        if (cp.graphKernelNodes.empty()) cp.graphAllEigen = false;
-                    }
-                    if (getenv("B200_BEAGLE_DEBUG"))
-                        fprintf(stderr, "[b200-beagle] graph %s: %d launches\n", cp.graphExec ? "captured" : "capture failed",
-                                launches);
-                    cudaGetLastError();
-                }
-                if (cp.graphExec != nullptr) {
-                    TimedScope ts(in, T_PARTIALS, launches);
-                    CUDA_OK(cudaGraphLaunch(cp.graphExec, in->stream));
-                    noteScaleWrites(in, hops);
-                    noteCherryWrites(in, hops, cp.cherries);
-                    return BEAGLE_SUCCESS;
-                }
-            }
-            CUDA_OK(launchPlan(in, cp.dBlock, static_cast<char*>(cp.dBlock) + cp.subsOffset, cp.phaseStart, cp.phaseSlots,
-                               cp.fourPath, cp.maxWindow, cp.preOrder, eigenSlot, !cp.byPartition, dSnap, nSnap, dTips));
-            CUDA_OK(accumulateInList(in, cp.cumGroups));
-            noteScaleWrites(in, hops);
-            noteCherryWrites(in, hops, cp.cherries);
-            return BEAGLE_SUCCESS;
-        }
-    }
-    {
-        const int rcPrepare = prepareOps(in, hops, byPartition);
-        if (rcPrepare != BEAGLE_SUCCESS) return rcPrepare;
-    }
+// planner parameters of a list over `window` patterns
+PlanParams planParams(const Instance* in, int window) {
     const bool fourState = in->matCP > 0;
-    const bool preOrder = hops[0].kind == 1;
-    const int eigenSlot = fourState ? eigenFormSlot(in, hops) : -1;
-    std::vector<char> written(in->nBuffers, 0);
-    std::vector<int> firstWrite(in->nBuffers, n);
-    for (int k = n - 1; k >= 0; --k) { written[hops[k].dest] = 1; firstWrite[hops[k].dest] = k; }
-    // ---- virtual cherries: the ops that are not run (each tip x tip op without rescaling whose destination this list
-    // writes once and reads only afterwards), and whether any op record names a virtual child
-    std::vector<CherryRef> cherries;
-    std::vector<int4> snap;
-    std::vector<HostOp> kept;
-    bool readsVirtual = false;
-    if (!in->cherryTip1.empty() && !byPartition && !preOrder && eigenSlot >= 0) {
-        std::vector<int> writes(in->nBuffers, 0), firstRead(in->nBuffers, n);
-        for (int k = 0; k < n; ++k) {
-            writes[hops[k].dest]++;
-            firstRead[hops[k].c1] = std::min(firstRead[hops[k].c1], k);
-            firstRead[hops[k].c2] = std::min(firstRead[hops[k].c2], k);
-        }
-        for (int k = 0; k < n; ++k) {
-            const HostOp& o = hops[k];
-            if (in->states8[o.c1] != nullptr && in->states8[o.c2] != nullptr && o.sw == BEAGLE_OP_NONE &&
-                o.sr == BEAGLE_OP_NONE && o.cum == BEAGLE_OP_NONE && writes[o.dest] == 1 && firstRead[o.dest] > k) {
-                cherries.push_back(CherryRef{o.dest, o.c1, o.c2});
-                snap.push_back(make_int4(o.dest, o.m1, o.m2, 0));
-            } else {
-                kept.push_back(o);
-            }
-        }
-        if (kept.empty()) { cherries.clear(); snap.clear(); }       // nothing would run: keep the list as it is
-        readsVirtual = !cherries.empty();
-        for (const HostOp& o : hops)
-            for (int c : {o.c1, o.c2})
-                readsVirtual = readsVirtual || (!written[c] && in->states32[c] == nullptr && in->cherryTip1[c] >= 0);
-    }
-    Plan plan;
-    int maxWindow = in->Ppad;
     // patterns one warp owns: 4-state kernels (32/CP)*R, S > 4 tensor kernel 16
     const int patsPerWarp = !fourState ? 16 : (32 / in->matCP) * in->walkR;
     const int warpsPerSM = fourState ? 32 : 12;      // resident warps the kernel family can hold per SM
-    auto wantSubsFor = [&](int window) {
-        const int warpsPerSub = std::max(1, (window + patsPerWarp - 1) / patsPerWarp);
-        // enough (subtree x tile) walks to fill every SM, oversubscribed for balance
-        // oversubscription for balance: 2x where a subtree is only a few warps wide (small alignments), 1x where every
-        // subtree already spreads over dozens of warps -- longer walks forward more results through registers
-        // (measured: cfg 2 +3 %, codon +5 %, benchmark2 +4 %; benchmark1-sized inputs -1..-3 % if forced to 1)
-        const int over = in->phaseOversub > 0 ? in->phaseOversub : (warpsPerSub >= 32 ? 1 : 2);
-        return std::max(1, over * ((in->smCount * warpsPerSM + warpsPerSub - 1) / warpsPerSub));
-    };
-    if (!byPartition && !preOrder) {
-        planPhases(cherries.empty() ? hops : kept, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(in->Ppad),
-                   in->phaseTmin, in->phaseSmall, plan);
-        // only k_walk4p reads virtual children: if some phase of this plan would run elsewhere, every op runs as usual
-        bool served = true;
-        for (size_t ph = 0; readsVirtual && ph + 1 < plan.phaseStart.size(); ++ph) {
-            const int nSubs = plan.phaseStart[ph + 1] - plan.phaseStart[ph];
-            served = served && (nSubs == 0 || walk4pServes(in, nSubs, in->Ppad));
-        }
-        if (!served) {
-            readsVirtual = false;
-            if (!cherries.empty()) {
-                cherries.clear(); snap.clear(); kept.clear();
-                planPhases(hops, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin,
-                           in->phaseSmall, plan);
-            }
-        }
-        for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
-    }
-    // the ops that run
-    const std::vector<HostOp>& L = cherries.empty() ? hops : kept;
-    const int nL = (int)L.size();
-    // children from outside the list -- read at or before the first op that writes them, which may come later in the list
-    // (such lists run in the caller's order): read as virtual cherries where the records can say so, i.e. when the list
-    // never writes them, else as stored partials
-    std::vector<int> vt1(readsVirtual ? in->nBuffers : 0, -1), vt2(readsVirtual ? in->nBuffers : 0, -1);
-    for (const CherryRef& c : cherries) { vt1[c.buf] = c.tip1; vt2[c.buf] = c.tip2; }
-    std::vector<CherryRef> external;
-    {
-        std::vector<char> seen(in->nBuffers, 0);
-        for (int k = 0; k < n; ++k)
-            for (int c : {hops[k].c1, hops[k].c2}) {
-                if (firstWrite[c] < k || in->states32[c] != nullptr || seen[c]) continue;
-                seen[c] = 1;
-                const bool virt = readsVirtual && !written[c] && in->cherryTip1[c] >= 0;
-                external.push_back(CherryRef{c, virt ? in->cherryTip1[c] : -1, virt ? in->cherryTip2[c] : -1});
-                if (virt) { vt1[c] = in->cherryTip1[c]; vt2[c] = in->cherryTip2[c]; }
-            }
-    }
-    CUDA_OK(storeExternal(in, external));
-    {
-        if (!byPartition) {
-            if (preOrder) {
-                if (in->prePhases) planPreorderPhases(hops, in->nBuffers, in->phaseT, wantSubsFor(in->Ppad), in->phaseTmin, in->phaseSmall, plan);
-                else planLevels(hops, in->nBuffers, plan);
-                for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
-            }
-        } else {
-            // partitions are independent (disjoint pattern windows): plan each one on its own and merge the
-            // plans phase by phase; every subtree carries its partition's pattern window
-            std::vector<std::vector<int>> members(in->partitionCount);
-            for (int k = 0; k < n; ++k) members[hops[k].part].push_back(k);
-            std::vector<Plan> plans;
-            std::vector<int> base;
-            maxWindow = 1;
-            for (int part = 0; part < in->partitionCount; ++part) {
-                if (members[part].empty()) continue;
-                std::vector<HostOp> sub(members[part].size());
-                for (size_t q = 0; q < sub.size(); ++q) sub[q] = hops[members[part][q]];
-                Plan pl;
-                const int window = in->partEnd[part] - in->partBegin[part];
-                if (sub[0].kind == 1 && in->prePhases) planPreorderPhases(sub, in->nBuffers, in->phaseT, wantSubsFor(std::max(1, window)), in->phaseTmin, in->phaseSmall, pl);
-                else if (sub[0].kind == 1) planLevels(sub, in->nBuffers, pl);
-                else planPhases(sub, in->nBuffers, in->reorder != 0, in->phaseT, wantSubsFor(std::max(1, window)), in->phaseTmin, in->phaseSmall, pl);
-                base.push_back((int)plan.order.size());
-                for (int idx : pl.order) plan.order.push_back(members[part][idx]);
-                for (Sub& sb : pl.subs) {
-                    sb.begin += base.back(); sb.end += base.back();
-                    sb.pBase = in->partBegin[part]; sb.pLimit = in->partEnd[part];
-                }
-                maxWindow = std::max(maxWindow, window);
-                plans.push_back(std::move(pl));
-            }
-            plan.phaseStart.assign(1, 0);
-            for (size_t ph = 0;; ++ph) {
-                bool any = false;
-                for (const Plan& pl : plans) {
-                    if (ph + 1 >= pl.phaseStart.size()) continue;
-                    any = true;
-                    for (int q = pl.phaseStart[ph]; q < pl.phaseStart[ph + 1]; ++q) plan.subs.push_back(pl.subs[q]);
-                }
-                if (!any) break;
-                plan.phaseStart.push_back((int)plan.subs.size());
-            }
-        }
-    }
-    const std::vector<int>& order = plan.order;
+    const int warpsPerSub = std::max(1, (window + patsPerWarp - 1) / patsPerWarp);
+    // enough (subtree x tile) walks to fill every SM, oversubscribed for balance: 2x where a subtree is only a few warps
+    // wide (small alignments), 1x where every subtree already spreads over dozens of warps -- longer walks forward more
+    // results through registers (measured: cfg 2 +3 %, codon +5 %, benchmark2 +4 %; benchmark1-sized inputs -1..-3 % if
+    // forced to 1)
+    const int over = in->phaseOversub > 0 ? in->phaseOversub : (warpsPerSub >= 32 ? 1 : 2);
+    const int wantSubs = std::max(1, over * ((in->smCount * warpsPerSM + warpsPerSub - 1) / warpsPerSub));
+    return PlanParams{in->phaseT, wantSubs, in->phaseTmin, in->phaseSmall, in->reorder != 0, in->prePhases != 0};
+}
 
-    const int nPhases = (int)plan.phaseStart.size() - 1;
-    std::vector<int> subOfPos(nL, 0);
-    for (int sIdx = 0; sIdx < (int)plan.subs.size(); ++sIdx)
-        for (int q = plan.subs[sIdx].begin; q < plan.subs[sIdx].end; ++q) subOfPos[q] = sIdx;
-
-    const bool fourPath = in->matCP > 0;
-    std::vector<CumGroup> cumGroups;
-    std::vector<DevOp> dops(fourPath ? 0 : nL);
-    std::vector<Op4> ops4(fourPath ? nL : 0);
-    std::vector<int4> virtTips(readsVirtual ? nL : 0);     // k_walk4pv: the tips of each op's virtual children
-    for (int pos = 0; pos < nL; ++pos) {
-        const HostOp& o = L[order[pos]];
-        const bool t1 = in->states32[o.c1] != nullptr;
-        const bool t2 = in->states32[o.c2] != nullptr;
-        const int pBegin = byPartition ? in->partBegin[o.part] : 0;
-        const int pEnd = byPartition ? in->partEnd[o.part] : in->P;
-        // In-list cumulative scaling (cumulativeScaleIndex != NONE) is NOT done inside the walk: independent subtrees of a
-        // phase run concurrently over the same pattern columns, so a "cum[p] += log m" there would race.  The walk only
-        // writes the per-node factors; one k_scale_accum launch per (cumulative buffer, pattern window) follows the phases.
-        if (o.cum >= 0 && o.sw >= 0) {
-            CumGroup* grp = nullptr;
-            for (CumGroup& g : cumGroups) if (g.cum == o.cum && g.pBegin == pBegin && g.pEnd == pEnd) { grp = &g; break; }
-            if (grp == nullptr) { cumGroups.push_back(CumGroup{o.cum, pBegin, pEnd, {}}); grp = &cumGroups.back(); }
-            grp->indices.push_back(o.sw);
-        }
-        const int cum = -1;
-        if (fourPath) {
-            Op4& d = ops4[pos];
-            // a virtual cherry child: its buffer index (recipe row) and its two tips
-            const bool v1 = readsVirtual && !t1 && vt1[o.c1] >= 0, v2 = readsVirtual && !t2 && vt1[o.c2] >= 0;
-            d.dest = in->slotOf[o.dest];
-            d.c1 = t1 ? -(o.c1 + 1) : v1 ? o.c1 : in->slotOf[o.c1];
-            d.c2 = t2 ? -(o.c2 + 1) : v2 ? o.c2 : in->slotOf[o.c2];
-            d.m1 = o.m1; d.m2 = o.m2; d.sw = o.sw; d.sr = o.sr; d.cum = cum;
-            d.pBegin = pBegin; d.pEnd = pEnd;
-            d.slots = 0xFFFFFFu;                              // no sibling-stack slots until assignStackSlots
-            d.pad_ = o.kind | (v1 ? 4 : 0) | (v2 ? 8 : 0);
-            d.pfA = d.pfB = 0; d.pfM1 = d.pfM2 = -1;
-            if (readsVirtual)
-                virtTips[pos] = make_int4(v1 ? vt1[o.c1] : 0, v1 ? vt2[o.c1] : 0, v2 ? vt1[o.c2] : 0, v2 ? vt2[o.c2] : 0);
-            if (in->forward && pos > plan.subs[subOfPos[pos]].begin)
-                forwardFromPrevious(d, ops4[pos - 1], preOrder, readsVirtual ? &virtTips[pos] : nullptr);
+// virtual cherries: the ops that are not run (each tip x tip op without rescaling whose destination this list writes once
+// and reads only afterwards) go to `cherries` and `snap`, the others to `kept`.  Returns whether any op record names a
+// virtual child.  firstWrite[b]: position of the list's first write of buffer b (n: none)
+bool selectCherries(const Instance* in, const std::vector<HostOp>& hops, const std::vector<int>& firstWrite,
+                    std::vector<CherryRef>& cherries, std::vector<int4>& snap, std::vector<HostOp>& kept) {
+    const int n = (int)hops.size();
+    std::vector<int> writes(in->nBuffers, 0), firstRead(in->nBuffers, n);
+    for (int k = 0; k < n; ++k) {
+        writes[hops[k].dest]++;
+        firstRead[hops[k].c1] = std::min(firstRead[hops[k].c1], k);
+        firstRead[hops[k].c2] = std::min(firstRead[hops[k].c2], k);
+    }
+    for (int k = 0; k < n; ++k) {
+        const HostOp& o = hops[k];
+        if (in->states8[o.c1] != nullptr && in->states8[o.c2] != nullptr && o.sw == BEAGLE_OP_NONE &&
+            o.sr == BEAGLE_OP_NONE && o.cum == BEAGLE_OP_NONE && writes[o.dest] == 1 && firstRead[o.dest] > k) {
+            cherries.push_back(CherryRef{o.dest, o.c1, o.c2});
+            snap.push_back(make_int4(o.dest, o.m1, o.m2, 0));
         } else {
-            DevOp& d = dops[pos];
-            memset(&d, 0, sizeof d);
-            d.dest = reinterpret_cast<double*>(in->partials[o.dest]);          // S > 4: always a double instance
-            d.c1 = t1 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c1]);
-            d.c2 = t2 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c2]);
-            d.s1 = t1 ? (const void*)in->states32[o.c1] : nullptr;
-            d.s2 = t2 ? (const void*)in->states32[o.c2] : nullptr;
-            d.m1 = in->dMat + (size_t)o.m1 * in->matStride;
-            d.m2 = in->dMat + (size_t)o.m2 * in->matStride;
-            d.scaleWrite = o.sw >= 0 ? in->dScale + (size_t)o.sw * in->Ppad : nullptr;
-            d.scaleRead = o.sr >= 0 ? in->dScale + (size_t)o.sr * in->Ppad : nullptr;
-            d.cumScale = cum >= 0 ? in->dScale + (size_t)cum * in->Ppad : nullptr;
-            d.pBegin = pBegin; d.pEnd = pEnd;
-            d.pad_ = o.kind;
-            // register forwarding on the tensor-pipe walk (one category): the warp that wrote the previous op's 16-pattern
-            // tile still holds it in its accumulators -- flag the child (moved to position 1; the product commutes exactly)
-            if (in->forward && !preOrder && pos > plan.subs[subOfPos[pos]].begin) {
-                const DevOp& pv = dops[pos - 1];
-                if (pv.pBegin == d.pBegin && pv.pEnd == d.pEnd) {
-                    if (d.c1 != nullptr && d.c1 == pv.dest) d.pad_ |= 2;
-                    else if (d.c2 != nullptr && d.c2 == pv.dest) {
-                        std::swap(d.c1, d.c2); std::swap(d.s1, d.s2); std::swap(d.m1, d.m2); d.pad_ |= 2;
-                    }
-                }
-            }
+            kept.push_back(o);
         }
     }
-    // sibling stack: lists whose phases the staged eigen walk may run (post-order, aligned)
-    std::vector<int> phaseSlots(std::max(nPhases, 1), 0);
-    long fromStack = 0, fromMemory = 0;
-    if (fourPath && eigenSlot >= 0 && !preOrder && !byPartition && in->stackSlots > 0 && walkStackBuilt(in)) {
-        std::vector<int> subDepth;
-        assignStackSlots(ops4, plan.subs, in->stackSlots, subDepth, fromStack, fromMemory);
-        for (int ph = 0; ph < nPhases; ++ph)
-            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) phaseSlots[ph] = std::max(phaseSlots[ph], subDepth[q]);
-    }
-    if (fourPath && in->lookahead && (!preOrder || in->lookaheadPre)) {
-        // look-ahead fields: what op k+1 of the same walk will read from memory, except op k's own destination
-        // only where the phase is throughput-bound; a thin phase is a pure latency chain and the extra instructions cost
-        // more than the prefetch gives (measured on the 62-taxon benchmark2 alignment: +17 % with, in thin phases)
-        std::vector<char> thick(plan.subs.size(), 0);
-        const long perSub = (maxWindow + (32 / in->matCP) * in->walkR - 1) / ((32 / in->matCP) * in->walkR);
-        for (int ph = 0; ph < nPhases; ++ph) {
-            const bool t = (long)(plan.phaseStart[ph + 1] - plan.phaseStart[ph]) * perSub >= (long)in->smCount * 8;
-            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) thick[q] = t;
+    if (kept.empty()) { cherries.clear(); snap.clear(); }       // nothing would run: keep the list as it is
+    bool readsVirtual = !cherries.empty();
+    for (const HostOp& o : hops)
+        for (int c : {o.c1, o.c2})
+            readsVirtual = readsVirtual || (firstWrite[c] == n && in->states32[c] == nullptr && in->cherryTip1[c] >= 0);
+    return readsVirtual;
+}
+
+// partitions are independent (disjoint pattern windows): plan each one on its own and merge the plans phase by phase;
+// every subtree carries its partition's pattern window.  Returns the widest window.
+int planPartitions(const Instance* in, const std::vector<HostOp>& hops, Plan& plan) {
+    std::vector<std::vector<int>> members(in->partitionCount);
+    for (int k = 0; k < (int)hops.size(); ++k) members[hops[k].part].push_back(k);
+    std::vector<Plan> plans;
+    int maxWindow = 1;
+    for (int part = 0; part < in->partitionCount; ++part) {
+        if (members[part].empty()) continue;
+        std::vector<HostOp> sub(members[part].size());
+        for (size_t q = 0; q < sub.size(); ++q) sub[q] = hops[members[part][q]];
+        Plan pl;
+        const int window = in->partEnd[part] - in->partBegin[part];
+        planList(sub, in->nBuffers, planParams(in, std::max(1, window)), pl);
+        const int base = (int)plan.order.size();
+        for (int idx : pl.order) plan.order.push_back(members[part][idx]);
+        for (Sub& sb : pl.subs) {
+            sb.begin += base; sb.end += base;
+            sb.pBase = in->partBegin[part]; sb.pLimit = in->partEnd[part];
         }
-        for (size_t sIdx = 0; sIdx < plan.subs.size(); ++sIdx) {
-            if (!thick[sIdx] && in->lookahead < 2) continue;
-            for (int pos = plan.subs[sIdx].begin; pos + 1 < plan.subs[sIdx].end; ++pos) {
-                Op4& d = ops4[pos];
-                const Op4& nx = ops4[pos + 1];
+        maxWindow = std::max(maxWindow, window);
+        plans.push_back(std::move(pl));
+    }
+    plan.phaseStart.assign(1, 0);
+    for (size_t ph = 0;; ++ph) {
+        bool any = false;
+        for (const Plan& pl : plans) {
+            if (ph + 1 >= pl.phaseStart.size()) continue;
+            any = true;
+            for (int q = pl.phaseStart[ph]; q < pl.phaseStart[ph + 1]; ++q) plan.subs.push_back(pl.subs[q]);
+        }
+        if (!any) break;
+        plan.phaseStart.push_back((int)plan.subs.size());
+    }
+    return maxWindow;
+}
+
+// the 4-state record of op o before forwarding, stack slots and look-ahead; vt: the tips of every virtual cherry the
+// records name, by buffer (empty: none); tips: where the tips of o's virtual children go (nullptr: none)
+void encodeOp4(const Instance* in, const HostOp& o, int pBegin, int pEnd, const std::vector<int2>& vt, Op4& d, int4* tips) {
+    const bool t1 = in->states32[o.c1] != nullptr, t2 = in->states32[o.c2] != nullptr;
+    const bool v1 = !vt.empty() && !t1 && vt[o.c1].x >= 0, v2 = !vt.empty() && !t2 && vt[o.c2].x >= 0;
+    d.dest = in->slotOf[o.dest];
+    d.c1 = t1 ? -(o.c1 + 1) : v1 ? o.c1 : in->slotOf[o.c1];     // a virtual cherry child: its buffer index (recipe row)
+    d.c2 = t2 ? -(o.c2 + 1) : v2 ? o.c2 : in->slotOf[o.c2];
+    d.m1 = o.m1; d.m2 = o.m2; d.sw = o.sw; d.sr = o.sr; d.cum = -1;
+    d.pBegin = pBegin; d.pEnd = pEnd;
+    d.slots = 0xFFFFFFu;                              // no sibling-stack slots until assignStackSlots
+    d.pad_ = o.kind | (v1 ? 4 : 0) | (v2 ? 8 : 0);
+    d.pfA = d.pfB = 0; d.pfM1 = d.pfM2 = -1;
+    if (tips) *tips = make_int4(v1 ? vt[o.c1].x : 0, v1 ? vt[o.c1].y : 0, v2 ? vt[o.c2].x : 0, v2 ? vt[o.c2].y : 0);
+}
+
+// the record of op o on the generic (S > 4) walk before forwarding; those instances are always double
+void encodeDevOp(const Instance* in, const HostOp& o, int pBegin, int pEnd, DevOp& d) {
+    const bool t1 = in->states32[o.c1] != nullptr, t2 = in->states32[o.c2] != nullptr;
+    memset(&d, 0, sizeof d);
+    d.dest = reinterpret_cast<double*>(in->partials[o.dest]);
+    d.c1 = t1 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c1]);
+    d.c2 = t2 ? nullptr : reinterpret_cast<const double*>(in->partials[o.c2]);
+    d.s1 = t1 ? (const void*)in->states32[o.c1] : nullptr;
+    d.s2 = t2 ? (const void*)in->states32[o.c2] : nullptr;
+    d.m1 = in->dMat + (size_t)o.m1 * in->matStride;
+    d.m2 = in->dMat + (size_t)o.m2 * in->matStride;
+    d.scaleWrite = o.sw >= 0 ? in->dScale + (size_t)o.sw * in->Ppad : nullptr;
+    d.scaleRead = o.sr >= 0 ? in->dScale + (size_t)o.sr * in->Ppad : nullptr;
+    d.cumScale = nullptr;
+    d.pBegin = pBegin; d.pEnd = pEnd;
+    d.pad_ = o.kind;
+}
+
+// look-ahead fields: what op k+1 of the same walk will read from memory, except op k's own destination
+// only where the phase is throughput-bound; a thin phase is a pure latency chain and the extra instructions cost
+// more than the prefetch gives (measured on the 62-taxon benchmark2 alignment: +17 % with, in thin phases)
+void setLookahead(const Instance* in, std::vector<Op4>& ops, const Plan& plan, int maxWindow) {
+    const long perSub = (maxWindow + (32 / in->matCP) * in->walkR - 1) / ((32 / in->matCP) * in->walkR);
+    for (size_t ph = 0; ph + 1 < plan.phaseStart.size(); ++ph) {
+        if ((long)(plan.phaseStart[ph + 1] - plan.phaseStart[ph]) * perSub < (long)in->smCount * 8) continue;
+        for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q)
+            for (int pos = plan.subs[q].begin; pos + 1 < plan.subs[q].end; ++pos) {
+                Op4& d = ops[pos];
+                const Op4& nx = ops[pos + 1];
                 auto enc = [&](int child, bool fromRegisters, bool virt, bool fromStack) -> int {
                     if (fromRegisters || virt || fromStack) return 0;
                     if (child < 0) return ((-child - 1) << 1) | 1;
@@ -1000,80 +840,289 @@ int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartitio
                 if (d.pfA == 0) { d.pfA = d.pfB; d.pfB = 0; }
                 d.pfM1 = nx.m1; d.pfM2 = nx.m2;
             }
-        }
     }
-    if (fourPath && getenv("B200_BEAGLE_DEBUG")) {
+}
+
+// A validated list -> its plan record and the host block [op records | subtree table | snapshot items | virtual tips],
+// each part 256-byte aligned; no CUDA calls.  eigenSlot: eigenFormSlot of the list.
+std::vector<char> buildPlan(const Instance* in, const std::vector<HostOp>& hops, bool byPartition, int eigenSlot,
+                            PlanRecord& r) {
+    const int n = (int)hops.size();
+    r.fourPath = in->matCP > 0;
+    r.preOrder = hops[0].kind == 1;
+    r.byPartition = byPartition;
+    std::vector<int> firstWrite(in->nBuffers, n);
+    for (int k = n - 1; k >= 0; --k) firstWrite[hops[k].dest] = k;
+    std::vector<int4> snap;
+    std::vector<HostOp> kept;
+    if (!in->cherryTip1.empty() && !byPartition && eigenSlot >= 0)
+        r.readsVirtual = selectCherries(in, hops, firstWrite, r.cherries, snap, kept);
+    Plan plan;
+    if (byPartition) {
+        r.maxWindow = planPartitions(in, hops, plan);
+    } else {
+        r.maxWindow = in->Ppad;
+        const PlanParams pp = planParams(in, in->Ppad);
+        planList(r.cherries.empty() ? hops : kept, in->nBuffers, pp, plan);
+        // only k_walk4p reads virtual children: if some phase of this plan would run elsewhere, every op runs as usual
+        bool served = true;
+        for (size_t ph = 0; r.readsVirtual && ph + 1 < plan.phaseStart.size(); ++ph) {
+            const int nSubs = plan.phaseStart[ph + 1] - plan.phaseStart[ph];
+            served = served && (nSubs == 0 || walk4pServes(in, nSubs, in->Ppad));
+        }
+        if (!served) {
+            r.readsVirtual = false;
+            if (!r.cherries.empty()) {
+                r.cherries.clear(); snap.clear(); kept.clear();
+                planList(hops, in->nBuffers, pp, plan);
+            }
+        }
+        for (Sub& sb : plan.subs) { sb.pBase = 0; sb.pLimit = in->Ppad; }
+    }
+    const std::vector<HostOp>& L = r.cherries.empty() ? hops : kept;      // the ops that run
+    const int nL = (int)L.size(), nPhases = (int)plan.phaseStart.size() - 1;
+    // children from outside the list -- read at or before the first op that writes them, which may come later in the list
+    // (such lists run in the caller's order): read as virtual cherries where the records can say so, i.e. when the list
+    // never writes them, else as stored partials.  vt: the tips of every virtual cherry the records name, by buffer
+    std::vector<int2> vt(r.readsVirtual ? in->nBuffers : 0, make_int2(-1, -1));
+    for (const CherryRef& c : r.cherries) vt[c.buf] = make_int2(c.tip1, c.tip2);
+    std::vector<char> seen(in->nBuffers, 0);
+    for (int k = 0; k < n; ++k)
+        for (int c : {hops[k].c1, hops[k].c2}) {
+            if (firstWrite[c] < k || in->states32[c] != nullptr || seen[c]) continue;
+            seen[c] = 1;
+            const bool virt = r.readsVirtual && firstWrite[c] == n && in->cherryTip1[c] >= 0;
+            r.external.push_back(CherryRef{c, virt ? in->cherryTip1[c] : -1, virt ? in->cherryTip2[c] : -1});
+            if (virt) vt[c] = make_int2(in->cherryTip1[c], in->cherryTip2[c]);
+        }
+    std::vector<DevOp> dops(r.fourPath ? 0 : nL);
+    std::vector<Op4> ops4(r.fourPath ? nL : 0);
+    std::vector<int4> virtTips(r.readsVirtual ? nL : 0);     // k_walk4pv: the tips of each op's virtual children
+    for (int pos = 0; pos < nL; ++pos) {
+        const HostOp& o = L[plan.order[pos]];
+        const int pBegin = byPartition ? in->partBegin[o.part] : 0, pEnd = byPartition ? in->partEnd[o.part] : in->P;
+        // In-list cumulative scaling (cumulativeScaleIndex != NONE) is NOT done inside the walk: independent subtrees of a
+        // phase run concurrently over the same pattern columns, so a "cum[p] += log m" there would race.  The walk only
+        // writes the per-node factors; one k_scale_accum launch per (cumulative buffer, pattern window) follows the phases.
+        if (o.cum >= 0 && o.sw >= 0) {
+            CumGroup* grp = nullptr;
+            for (CumGroup& g : r.cumGroups) if (g.cum == o.cum && g.pBegin == pBegin && g.pEnd == pEnd) { grp = &g; break; }
+            if (grp == nullptr) { r.cumGroups.push_back(CumGroup{o.cum, pBegin, pEnd, {}}); grp = &r.cumGroups.back(); }
+            grp->indices.push_back(o.sw);
+        }
+        if (r.fourPath) encodeOp4(in, o, pBegin, pEnd, vt, ops4[pos], virtTips.empty() ? nullptr : &virtTips[pos]);
+        else encodeDevOp(in, o, pBegin, pEnd, dops[pos]);
+    }
+    if (in->forward && r.fourPath) forwardOps4(ops4, plan.subs, r.preOrder, virtTips.empty() ? nullptr : virtTips.data());
+    if (in->forward && !r.fourPath && !r.preOrder) forwardDevOps(dops, plan.subs);
+    // sibling stack: lists whose phases the staged eigen walk may run (post-order, aligned)
+    r.phaseStart = plan.phaseStart;
+    r.phaseSlots.assign(std::max(nPhases, 1), 0);
+    long fromStack = 0, fromMemory = 0;
+    if (eigenSlot >= 0 && !byPartition && in->stackSlots > 0 && walkStackBuilt(in)) {
+        std::vector<int> subDepth;
+        assignStackSlots(ops4, plan.subs, in->stackSlots, subDepth, fromStack, fromMemory);
+        for (int ph = 0; ph < nPhases; ++ph)
+            for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q) r.phaseSlots[ph] = std::max(r.phaseSlots[ph], subDepth[q]);
+    }
+    if (r.fourPath && (!r.preOrder || in->lookaheadPre)) setLookahead(in, ops4, plan, r.maxWindow);
+    if (r.fourPath && in->debugLog) {
         int fwd = 0, internal = 0;
         for (const Op4& d : ops4) { fwd += (d.pad_ & 2) != 0; internal += (d.c1 >= 0) + (d.c2 >= 0); }
         fprintf(stderr, "[b200-beagle] plan: %d ops (%zu virtual cherries), %zu subtrees, %d phases, %d internal children, "
-                "%d forwarded in registers, %ld read from the stack, %ld from memory\n", nL, cherries.size(), plan.subs.size(),
+                "%d forwarded in registers, %ld read from the stack, %ld from memory\n", nL, r.cherries.size(), plan.subs.size(),
                 nPhases, internal, fwd, fromStack, fromMemory);
     }
-    // one block: [op records | subtree table | snapshot items], each part 256-byte aligned
-    const size_t opBytes = (fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)nL;
+    auto aligned = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
+    const size_t opBytes = (r.fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)nL;
     const size_t subBytes = sizeof(Sub) * plan.subs.size();
     const size_t snapBytes = sizeof(int4) * snap.size();
-    const size_t subsOffset = (opBytes + 255) & ~size_t(255);
-    const size_t snapOffset = subsOffset + ((subBytes + 255) & ~size_t(255));
     const size_t tipsBytes = sizeof(int4) * virtTips.size();
-    const size_t tipsOffset = snapOffset + ((snapBytes + 255) & ~size_t(255));
-    const size_t blockBytes = tipsOffset + tipsBytes;
-    std::vector<char> hBlock(blockBytes, 0);
-    memcpy(hBlock.data(), fourPath ? (const void*)ops4.data() : (const void*)dops.data(), opBytes);
-    memcpy(hBlock.data() + subsOffset, plan.subs.data(), subBytes);
-    if (snapBytes) memcpy(hBlock.data() + snapOffset, snap.data(), snapBytes);
-    if (tipsBytes) memcpy(hBlock.data() + tipsOffset, virtTips.data(), tipsBytes);
-    void* dOps = stage(in, hBlock.data(), blockBytes);
+    r.subsOffset = aligned(opBytes);
+    r.snapOffset = r.subsOffset + aligned(subBytes);
+    r.tipsOffset = r.snapOffset + aligned(snapBytes);
+    r.bytes = r.tipsOffset + tipsBytes;
+    std::vector<char> block(r.bytes, 0);
+    memcpy(block.data(), r.fourPath ? (const void*)ops4.data() : (const void*)dops.data(), opBytes);
+    memcpy(block.data() + r.subsOffset, plan.subs.data(), subBytes);
+    if (snapBytes) memcpy(block.data() + r.snapOffset, snap.data(), snapBytes);
+    if (tipsBytes) memcpy(block.data() + r.tipsOffset, virtTips.data(), tipsBytes);
+    return block;
+}
+
+// run a plan from its device block -- as its captured graph when `graph` is non-null -- then its in-list cumulative
+// scaling, and note what the list wrote
+cudaError_t runPlan(Instance* in, const std::vector<HostOp>& hops, const PlanRecord& r, const void* dBlock, int eigenSlot,
+                    cudaGraphExec_t graph = nullptr) {
+    cudaError_t e;
+    if (graph != nullptr) {
+        TimedScope ts(in, T_PARTIALS, launchCount(r));
+        e = cudaGraphLaunch(graph, in->stream);
+    } else {
+        e = launchPlan(in, r, dBlock, eigenSlot);
+    }
+    if (e == cudaSuccess) e = accumulateInList(in, r.cumGroups);
+    if (e != cudaSuccess) return e;
+    noteScaleWrites(in, hops);
+    noteCherryWrites(in, hops, r.cherries);
+    return cudaSuccess;
+}
+
+// The graph a cache hit replays, or nullptr for plain launches.  A plan that keeps coming back and needs several dependent
+// launches is replayed as ONE graph launch: on small alignments the host-side launch cost, not the kernels, sets the pace.
+cudaGraphExec_t planGraph(Instance* in, CachedPlan& cp, int eigenSlot) {
+    const unsigned eigenGenNow = eigenSlot >= 0 ? in->eigenGen[eigenSlot] : 0u;
+    // a captured graph carries the kernel choice and V / V^-1 by value: stale once the eigen system moved on
+    if (cp.graphExec != nullptr && (cp.graphEigen != eigenSlot || cp.graphEigenGen != eigenGenNow)) {
+        // same kernels, new V / V^-1 (a substitution-model move): patch the captured launches in place
+        if (cp.graphAllEigen && eigenSlot >= 0 && cp.graphEigen == eigenSlot &&
+            updateWalk4EGraph(cp.graphExec, cp.graphKernelNodes, in->hEigen.data() + (size_t)eigenSlot * 36) == cudaSuccess) {
+            cp.graphEigenGen = eigenGenNow;
+        } else {
+            cudaGetLastError();
+            cp.dropGraph();
+            cp.hits = 1;
+            if (++cp.graphInvalidations >= 4) cp.graphFailed = true;     // the kernel choice flips every step: plain launches
+        }
+    }
+    const int launches = launchCount(cp.rec);
+    // (in-list cumulative scaling stages its index lists per call: those plans keep the plain launches)
+    if (!in->useGraphs || launches < 2 || !cp.rec.cumGroups.empty()) return nullptr;
+    if (cp.graphExec == nullptr && !cp.graphFailed && cp.hits >= 2 && !in->timing &&
+        cudaStreamBeginCapture(in->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+        const cudaError_t e1 = launchPlan(in, cp.rec, cp.dBlock, eigenSlot);
+        cp.graphEigen = eigenSlot;
+        cp.graphEigenGen = eigenGenNow;
+        cudaGraph_t g = nullptr;
+        const cudaError_t e2 = cudaStreamEndCapture(in->stream, &g);
+        if (e1 != cudaSuccess || e2 != cudaSuccess || g == nullptr || cudaGraphInstantiate(&cp.graphExec, g, 0) != cudaSuccess) {
+            cp.graphExec = nullptr;
+            cp.graphFailed = true;
+            if (g) cudaGraphDestroy(g);
+        } else {
+            cp.graph = g;
+            size_t nn = 0;
+            if (cudaGraphGetNodes(g, nullptr, &nn) == cudaSuccess && nn > 0) {
+                std::vector<cudaGraphNode_t> nodes(nn);
+                cudaGraphNodeType ty;
+                if (cudaGraphGetNodes(g, nodes.data(), &nn) == cudaSuccess)
+                    for (size_t q = 0; q < nn; ++q)
+                        if (cudaGraphNodeGetType(nodes[q], &ty) == cudaSuccess && ty == cudaGraphNodeTypeKernel)
+                            cp.graphKernelNodes.push_back(nodes[q]);
+            }
+            cp.graphAllEigen = eigenSlot >= 0 && !cp.graphKernelNodes.empty();
+        }
+        if (in->debugLog)
+            fprintf(stderr, "[b200-beagle] graph %s: %d launches\n", cp.graphExec ? "captured" : "capture failed", launches);
+        cudaGetLastError();
+    }
+    return cp.graphExec;
+}
+
+// remember a plan that ran from the staging ring: a device copy of its block (stream-ordered D2D) and its record, in the
+// first empty slot, else in place of the least recently used entry
+void rememberPlan(Instance* in, const std::vector<HostOp>& hops, PlanRecord&& rec, const void* dBlock) {
+    if ((int)in->planCache.size() < in->planCacheSize) in->planCache.emplace_back();
+    CachedPlan* slot = nullptr;
+    for (CachedPlan& cp : in->planCache) {
+        if (cp.dBlock == nullptr || cp.n < 0) { slot = &cp; break; }
+        if (slot == nullptr || cp.lastUse < slot->lastUse) slot = &cp;
+    }
+    slot->dropGraph();
+    if (slot->capacity < rec.bytes) {
+        if (slot->dBlock) cudaFree(slot->dBlock);
+        slot->dBlock = nullptr; slot->capacity = 0;
+        if (cudaMalloc(&slot->dBlock, rec.bytes) == cudaSuccess) slot->capacity = rec.bytes; else cudaGetLastError();
+    }
+    if (slot->dBlock != nullptr &&
+        cudaMemcpyAsync(slot->dBlock, dBlock, rec.bytes, cudaMemcpyDeviceToDevice, in->stream) == cudaSuccess) {
+        slot->key = hops; slot->n = (int)hops.size(); slot->epoch = in->bufferEpoch;
+        slot->lastUse = ++in->planClock;
+        slot->hits = 0; slot->graphInvalidations = 0;
+        slot->graphFailed = !rec.cumGroups.empty();      // the accumulate launches stage fresh index arrays: never captured
+        slot->rec = std::move(rec);
+    } else if (slot->dBlock != nullptr) {
+        slot->n = -1;
+    }
+}
+
+int planAndLaunch(Instance* in, const std::vector<HostOp>& hops, bool byPartition) {
+    const int n = (int)hops.size();
+    if (n == 0) return BEAGLE_SUCCESS;
+    // ---- plan cache: MCMC re-issues identical lists all the time (every move that keeps the topology and
+    // dirties all nodes, in BEAST's two buffer-index parities); a hit skips validation, planning and the H2D copy.
+    static_assert(sizeof(HostOp) == 10 * sizeof(int), "HostOp is compared bytewise");
+    for (CachedPlan& cp : in->planCache) {
+        if (cp.dBlock == nullptr || cp.n != n || cp.rec.byPartition != byPartition || cp.epoch != in->bufferEpoch ||
+            memcmp(cp.key.data(), hops.data(), sizeof(HostOp) * (size_t)n) != 0)
+            continue;
+        const int eigenSlot = eigenFormSlot(in, hops);
+        // records that name virtual cherries need the eigen form, and an outside child read as a cherry must still be it
+        bool stale = cp.rec.readsVirtual && eigenSlot < 0;
+        for (const CherryRef& x : cp.rec.external)
+            stale = stale || (x.tip1 >= 0 && (in->cherryTip1[x.buf] != x.tip1 || in->cherryTip2[x.buf] != x.tip2));
+        if (stale) { cp.dropGraph(); cp.n = -1; continue; }
+        CUDA_OK(storeExternal(in, cp.rec.external));
+        cp.lastUse = ++in->planClock;
+        cp.hits++;
+        CUDA_OK(runPlan(in, hops, cp.rec, cp.dBlock, eigenSlot, planGraph(in, cp, eigenSlot)));
+        return BEAGLE_SUCCESS;
+    }
+    const int rc = prepareOps(in, hops, byPartition);
+    if (rc != BEAGLE_SUCCESS) return rc;
+    const int eigenSlot = eigenFormSlot(in, hops);
+    PlanRecord rec;
+    const std::vector<char> hBlock = buildPlan(in, hops, byPartition, eigenSlot, rec);
+    CUDA_OK(storeExternal(in, rec.external));
+    void* dBlock = stage(in, hBlock.data(), rec.bytes);
     void* tmp = nullptr;
-    if (dOps == nullptr) {
+    if (dBlock == nullptr) {
         // list larger than the staging ring: one-off allocation
-        CUDA_OK(cudaMalloc(&tmp, blockBytes));
-        dOps = tmp;
-        cudaError_t ce = cudaMemcpyAsync(dOps, hBlock.data(), blockBytes, cudaMemcpyHostToDevice, in->stream);
+        CUDA_OK(cudaMalloc(&tmp, rec.bytes));
+        dBlock = tmp;
+        cudaError_t ce = cudaMemcpyAsync(dBlock, hBlock.data(), rec.bytes, cudaMemcpyHostToDevice, in->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(in->stream);
         if (ce != cudaSuccess) { cudaFree(tmp); CUDA_OK(ce); }
     }
-    void* dSubs = static_cast<char*>(dOps) + subsOffset;
-    cudaError_t e = launchPlan(in, dOps, dSubs, plan.phaseStart, phaseSlots, fourPath, maxWindow, preOrder, eigenSlot, !byPartition,
-                               static_cast<char*>(dOps) + snapOffset, (int)snap.size(),
-                               readsVirtual ? static_cast<char*>(dOps) + tipsOffset : nullptr);
-    if (e == cudaSuccess) e = accumulateInList(in, cumGroups);
-    noteScaleWrites(in, hops);
-    if (e == cudaSuccess) noteCherryWrites(in, hops, cherries);
-    if (e == cudaSuccess && tmp == nullptr && in->planCacheSize > 0) {
-        // remember the plan: device copy of the records (stream-ordered D2D out of the staging ring)
-        if ((int)in->planCache.size() < in->planCacheSize) in->planCache.emplace_back();
-        CachedPlan* slot = nullptr;            // first empty slot, else the least recently used entry
-        for (CachedPlan& cp : in->planCache) {
-            if (cp.dBlock == nullptr || cp.n < 0) { slot = &cp; break; }
-            if (slot == nullptr || cp.lastUse < slot->lastUse) slot = &cp;
-        }
-        slot->dropGraph();
-        slot->hits = 0;
-        slot->graphFailed = false;
-        slot->graphInvalidations = 0;
-        if (slot->capacity < blockBytes) {
-            if (slot->dBlock) cudaFree(slot->dBlock);
-            slot->dBlock = nullptr; slot->capacity = 0;
-            if (cudaMalloc(&slot->dBlock, blockBytes) == cudaSuccess) slot->capacity = blockBytes; else cudaGetLastError();
-        }
-        if (slot->dBlock != nullptr &&
-            cudaMemcpyAsync(slot->dBlock, dOps, blockBytes, cudaMemcpyDeviceToDevice, in->stream) == cudaSuccess) {
-            slot->key = hops; slot->n = n; slot->byPartition = byPartition; slot->epoch = in->bufferEpoch;
-            slot->subsOffset = subsOffset; slot->snapOffset = snapOffset; slot->tipsOffset = tipsOffset;
-            slot->cherries = cherries; slot->external = external; slot->readsVirtual = readsVirtual;
-            slot->phaseStart = plan.phaseStart; slot->phaseSlots = phaseSlots;
-            slot->fourPath = fourPath; slot->maxWindow = maxWindow; slot->preOrder = preOrder;
-            slot->lastUse = ++in->planClock;
-            slot->cumGroups = cumGroups;
-            slot->graphFailed = !cumGroups.empty();      // the accumulate launches stage fresh index arrays: never captured
-        } else if (slot->dBlock != nullptr) {
-            slot->n = -1;
-        }
-    }
+    const cudaError_t e = runPlan(in, hops, rec, dBlock, eigenSlot);
+    if (e == cudaSuccess && tmp == nullptr && in->planCacheSize > 0) rememberPlan(in, hops, std::move(rec), dBlock);
     if (tmp != nullptr) { cudaStreamSynchronize(in->stream); cudaFree(tmp); }
     CUDA_OK(e);
     return BEAGLE_SUCCESS;
+}
+
+// the caller's operations as HostOps (kind 1 = pre-order); a by-partition list names each op's cumulative scale buffer
+template <typename Op>
+std::vector<HostOp> hostOps(const Op* operations, int count, int kind, int cumulativeScaleIndex = BEAGLE_OP_NONE) {
+    std::vector<HostOp> hops(count);
+    for (int k = 0; k < count; ++k) {
+        const Op& o = operations[k];
+        hops[k] = {o.destinationPartials, o.destinationScaleWrite, o.destinationScaleRead, o.child1Partials,
+                   o.child1TransitionMatrix, o.child2Partials, o.child2TransitionMatrix, 0, cumulativeScaleIndex, kind};
+        if constexpr (std::is_same_v<Op, BeagleOperationByPartition>) {
+            hops[k].part = o.partition;
+            hops[k].cum = o.cumulativeScaleIndex;
+        }
+    }
+    return hops;
+}
+
+// the test hooks' common part: plan a 7-int-per-op list, report its subtrees and phases; false: an index out of range
+bool debugPlan(const int* operations, int count, int bufferCount, int kind, const PlanParams& pp, std::vector<HostOp>& hops,
+               Plan& plan, int* outSubs, int* outPhaseStart, int* outCounts) {
+    hops.resize(count);
+    for (int k = 0; k < count; ++k) {
+        const int* o = operations + 7 * k;
+        for (int f : {o[0], o[3], o[5]}) if (f < 0 || f >= bufferCount) return false;
+        hops[k] = {o[0], o[1], o[2], o[3], o[4], o[5], o[6], 0, -1, kind};
+    }
+    if (count == 0) { outCounts[0] = outCounts[1] = 0; return true; }
+    planList(hops, bufferCount, pp, plan);
+    for (size_t q = 0; q < plan.subs.size(); ++q) { outSubs[2 * q] = plan.subs[q].begin; outSubs[2 * q + 1] = plan.subs[q].end; }
+    for (size_t q = 0; q < plan.phaseStart.size(); ++q) outPhaseStart[q] = plan.phaseStart[q];
+    outCounts[0] = (int)plan.subs.size();
+    outCounts[1] = (int)plan.phaseStart.size() - 1;
+    return true;
 }
 
 }  // namespace
@@ -1211,12 +1260,10 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->hEigen.assign((size_t)std::max(1, in->nEigen) * 36, 0.0);
     in->eigenWalk = envInt("B200_EIGEN_WALK", 1);
     in->virtualCherries = envInt("B200_VIRTUAL_CHERRIES", 1);
-    in->walkBlock = 128;
     in->reorder = envInt("B200_REORDER", 1);
     in->forward = envInt("B200_FORWARD", 1);
     in->stackSlots = envInt("B200_WALK_STACK_SLOTS", 1) != 0 ? kStackSlots : 0;
     in->debugLog = getenv("B200_BEAGLE_DEBUG") != nullptr;
-    in->lookahead = envInt("B200_LOOKAHEAD", 1);
     in->useGraphs = envInt("B200_GRAPHS", 1);
     in->prePhases = envInt("B200_PRE_PHASES", 1);
     in->lookaheadPre = envInt("B200_LOOKAHEAD_PRE", 1);
@@ -1226,9 +1273,8 @@ int beagleCreateInstance(int tipCount, int partialsBufferCount, int compactBuffe
     in->phaseT = envInt("B200_PHASE_T", 0);
     in->phaseTmin = std::max(1, envInt("B200_PHASE_TMIN", 4));
     in->phaseSmall = envInt("B200_PHASE_SMALL", 24);
-    in->phaseOversub = std::max(0, envInt("B200_PHASE_OVERSUB", 0));      // 0 = by subtree width (see wantSubsFor)
+    in->phaseOversub = std::max(0, envInt("B200_PHASE_OVERSUB", 0));      // 0 = by subtree width (see planParams)
     in->genericMma = envInt("B200_GENERIC_MMA", 1);
-    in->mmaWarps = envInt("B200_MMA_WARPS", 4) == 8 ? 8 : 4;     // 8 = 256-thread blocks with cp.async double buffering
     // the SM count sizes the walk below: query the device first
     cudaDeviceProp prop;
     bool ok = cudaGetDeviceProperties(&prop, in->device) == cudaSuccess;
@@ -1917,12 +1963,7 @@ int beagleUpdatePartials(int instance, const BeagleOperation* operations, int op
     SH(instance, shBroadcast(sh, [&](int c) { return beagleUpdatePartials(c, operations, operationCount, cumulativeScaleIndex); }));
     GET_INSTANCE_LAZY(in, instance);
     if (operationCount < 0) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const BeagleOperation& o = operations[k];
-        hops[k] = {o.destinationPartials, o.destinationScaleWrite, o.destinationScaleRead, o.child1Partials,
-                   o.child1TransitionMatrix, o.child2Partials, o.child2TransitionMatrix, 0, cumulativeScaleIndex};
-    }
+    const std::vector<HostOp> hops = hostOps(operations, operationCount, 0, cumulativeScaleIndex);
     // a short list in eigen form: hold it back, calculateRootLogLikelihoods will run matrices + list + root as ONE launch
     if (fusionPossible(in) && operationCount >= 1 && operationCount <= kIncMaxOps && in->pendingOps.empty() &&
         cumulativeScaleIndex == BEAGLE_OP_NONE) {
@@ -1953,14 +1994,7 @@ int beagleUpdatePartialsByPartition(int instance, const BeagleOperationByPartiti
     SH(instance, BEAGLE_ERROR_NO_IMPLEMENTATION);
     GET_INSTANCE(in, instance);
     if (operationCount < 0) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const BeagleOperationByPartition& o = operations[k];
-        hops[k] = {o.destinationPartials, o.destinationScaleWrite, o.destinationScaleRead, o.child1Partials,
-                   o.child1TransitionMatrix, o.child2Partials, o.child2TransitionMatrix, o.partition,
-                   o.cumulativeScaleIndex};
-    }
-    return planAndLaunch(in, hops, true);
+    return planAndLaunch(in, hostOps(operations, operationCount, 0), true);
 }
 
 int beagleWaitForPartials(int instance, const int*, int) {
@@ -1974,28 +2008,13 @@ int beagleUpdatePrePartials(int instance, const BeagleOperation* operations, int
     SH(instance, shBroadcast(sh, [&](int c) { return beagleUpdatePrePartials(c, operations, operationCount, cumulativeScaleIndex); }));
     GET_INSTANCE(in, instance);
     if (operationCount < 0) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const BeagleOperation& o = operations[k];
-        hops[k] = {o.destinationPartials, o.destinationScaleWrite, o.destinationScaleRead, o.child1Partials,
-                   o.child1TransitionMatrix, o.child2Partials, o.child2TransitionMatrix, 0, cumulativeScaleIndex};
-        hops[k].kind = 1;
-    }
-    return planAndLaunch(in, hops, false);
+    return planAndLaunch(in, hostOps(operations, operationCount, 1, cumulativeScaleIndex), false);
 }
 int beagleUpdatePrePartialsByPartition(int instance, const BeagleOperationByPartition* operations, int operationCount) {
     SH(instance, BEAGLE_ERROR_NO_IMPLEMENTATION);
     GET_INSTANCE(in, instance);
     if (operationCount < 0) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const BeagleOperationByPartition& o = operations[k];
-        hops[k] = {o.destinationPartials, o.destinationScaleWrite, o.destinationScaleRead, o.child1Partials,
-                   o.child1TransitionMatrix, o.child2Partials, o.child2TransitionMatrix, o.partition,
-                   o.cumulativeScaleIndex};
-        hops[k].kind = 1;
-    }
-    return planAndLaunch(in, hops, true);
+    return planAndLaunch(in, hostOps(operations, operationCount, 1), true);
 }
 
 // ---- scale factors ----------------------------------------------------------------------------
@@ -2297,52 +2316,36 @@ int beagleCalculateCrossProductDerivative(int instance, const int* postBufferInd
 // ---- host-logic test hook (no CUDA calls): the execution plan of an operation list -----------------
 int b200DebugPlan(const int* operations, int operationCount, int bufferCount, int fixedT, int wantSubs, int minT,
                   int smallRemainder, int preOrder, int* outOrder, int* outSubs, int* outPhaseStart, int* outCounts) {
-    if (operationCount < 0 || bufferCount <= 0) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const int* o = operations + 7 * k;
-        for (int f : {o[0], o[3], o[5]}) if (f < 0 || f >= bufferCount) return BEAGLE_ERROR_OUT_OF_RANGE;
-        hops[k] = {o[0], o[1], o[2], o[3], o[4], o[5], o[6], 0, -1};
-        hops[k].kind = preOrder ? 1 : 0;
-    }
+    std::vector<HostOp> hops;
     Plan plan;
-    if (operationCount == 0) { outCounts[0] = outCounts[1] = 0; return BEAGLE_SUCCESS; }
-    if (preOrder == 2) planLevels(hops, bufferCount, plan);
-    else if (preOrder) planPreorderPhases(hops, bufferCount, fixedT, std::max(1, wantSubs), std::max(1, minT), smallRemainder, plan);
-    else planPhases(hops, bufferCount, true, fixedT, std::max(1, wantSubs), std::max(1, minT), smallRemainder, plan);
+    const PlanParams pp{fixedT, std::max(1, wantSubs), std::max(1, minT), smallRemainder, true, preOrder != 2};
+    if (operationCount < 0 || bufferCount <= 0 ||
+        !debugPlan(operations, operationCount, bufferCount, preOrder ? 1 : 0, pp, hops, plan, outSubs, outPhaseStart, outCounts))
+        return BEAGLE_ERROR_OUT_OF_RANGE;
     for (int k = 0; k < operationCount; ++k) outOrder[k] = plan.order[k];
-    for (size_t q = 0; q < plan.subs.size(); ++q) { outSubs[2 * q] = plan.subs[q].begin; outSubs[2 * q + 1] = plan.subs[q].end; }
-    for (size_t q = 0; q < plan.phaseStart.size(); ++q) outPhaseStart[q] = plan.phaseStart[q];
-    outCounts[0] = (int)plan.subs.size();
-    outCounts[1] = (int)plan.phaseStart.size() - 1;
     return BEAGLE_SUCCESS;
 }
 
 // ---- host-logic test hook (no CUDA calls): register forwarding and sibling-stack slots of a post-order list -----------
 int b200DebugStackSlots(const int* operations, int operationCount, int bufferCount, int tipCount, int wantSubs, int minT,
                         int smallRemainder, int* outRecords, int* outSubs, int* outPhaseStart, int* outCounts) {
-    if (operationCount <= 0 || bufferCount <= 0 || tipCount < 0 || tipCount > bufferCount) return BEAGLE_ERROR_OUT_OF_RANGE;
-    std::vector<HostOp> hops(operationCount);
-    for (int k = 0; k < operationCount; ++k) {
-        const int* o = operations + 7 * k;
-        for (int f : {o[0], o[3], o[5]}) if (f < 0 || f >= bufferCount) return BEAGLE_ERROR_OUT_OF_RANGE;
-        hops[k] = {o[0], o[1], o[2], o[3], o[4], o[5], o[6], 0, -1};
-    }
+    std::vector<HostOp> hops;
     Plan plan;
-    planPhases(hops, bufferCount, true, 0, std::max(1, wantSubs), std::max(1, minT), smallRemainder, plan);
+    const PlanParams pp{0, std::max(1, wantSubs), std::max(1, minT), smallRemainder, true, true};
+    if (operationCount <= 0 || bufferCount <= 0 || tipCount < 0 || tipCount > bufferCount ||
+        !debugPlan(operations, operationCount, bufferCount, 0, pp, hops, plan, outSubs, outPhaseStart, outCounts))
+        return BEAGLE_ERROR_OUT_OF_RANGE;
     std::vector<Op4> ops(operationCount);
     for (int pos = 0; pos < operationCount; ++pos) {            // buffers below tipCount are compact tips
         const HostOp& o = hops[plan.order[pos]];
         Op4& d = ops[pos];
-        memset(&d, 0, sizeof d);
         d.dest = o.dest;
         d.c1 = o.c1 < tipCount ? -(o.c1 + 1) : o.c1;
         d.c2 = o.c2 < tipCount ? -(o.c2 + 1) : o.c2;
         d.m1 = o.m1; d.m2 = o.m2; d.pEnd = 1;
         d.slots = 0xFFFFFFu;
     }
-    for (size_t s = 0; s < plan.subs.size(); ++s)
-        for (int pos = plan.subs[s].begin + 1; pos < plan.subs[s].end; ++pos) forwardFromPrevious(ops[pos], ops[pos - 1], false, nullptr);
+    forwardOps4(ops, plan.subs, false, nullptr);
     std::vector<int> subDepth;
     long fromStack = 0, fromMemory = 0;
     assignStackSlots(ops, plan.subs, kStackSlots, subDepth, fromStack, fromMemory);
@@ -2351,10 +2354,6 @@ int b200DebugStackSlots(const int* operations, int operationCount, int bufferCou
         int* r = outRecords + 5 * pos;
         r[0] = d.dest; r[1] = d.c1; r[2] = d.c2; r[3] = d.pad_; r[4] = (int)d.slots;
     }
-    for (size_t q = 0; q < plan.subs.size(); ++q) { outSubs[2 * q] = plan.subs[q].begin; outSubs[2 * q + 1] = plan.subs[q].end; }
-    for (size_t q = 0; q < plan.phaseStart.size(); ++q) outPhaseStart[q] = plan.phaseStart[q];
-    outCounts[0] = (int)plan.subs.size();
-    outCounts[1] = (int)plan.phaseStart.size() - 1;
     outCounts[2] = (int)fromStack;
     outCounts[3] = (int)fromMemory;
     outCounts[4] = *std::max_element(subDepth.begin(), subDepth.end());

@@ -66,21 +66,27 @@ using EdgeRef = EdgeRefT<double>;
 struct HostOp { int dest, sw, sr, c1, m1, c2, m2, part, cum; int kind = 0; };   // kind 1 = pre-order op
 // in-list cumulative scaling of an updatePartials call: cum[p] += sum over `indices` of log factor[p] on [pBegin, pEnd)
 struct CumGroup { int cum, pBegin, pEnd; std::vector<int> indices; };
-struct CachedPlan {
-    std::vector<HostOp> key;
-    std::vector<CumGroup> cumGroups;
-    int n = -1;
-    bool byPartition = false, fourPath = false, preOrder = false;
-    unsigned long epoch = 0;
-    // [op records | subtree table | snapshot items of the virtual cherries | tips of the virtual children per op]
-    void* dBlock = nullptr;
-    size_t capacity = 0, subsOffset = 0, snapOffset = 0, tipsOffset = 0;
+// what launching a planned list needs besides its block
+// [op records | subtree table | snapshot items of the virtual cherries | tips of the virtual children per op]
+struct PlanRecord {
+    std::vector<int> phaseStart, phaseSlots;      // phaseSlots: sibling-stack depth per phase
+    bool fourPath = false, preOrder = false;
+    bool byPartition = false;                     // false: aligned, every op covers [0, Ppad)
+    int maxWindow = 0;
+    size_t bytes = 0, subsOffset = 0, snapOffset = 0, tipsOffset = 0;
     // virtual cherries: the ones the list produces (not run; their recipes are snapshot first), and the children read from
     // outside the list -- as a virtual cherry (tip1 >= 0, must still be that cherry on a hit) or as stored partials
     std::vector<CherryRef> cherries, external;
     bool readsVirtual = false;                // some op record names a virtual child: needs the eigen form
-    std::vector<int> phaseStart, phaseSlots;      // phaseSlots: sibling-stack depth per phase
-    int maxWindow = 0;
+    std::vector<CumGroup> cumGroups;
+};
+struct CachedPlan {
+    std::vector<HostOp> key;
+    PlanRecord rec;
+    int n = -1;
+    unsigned long epoch = 0;
+    void* dBlock = nullptr;                   // device copy of the plan's block
+    size_t capacity = 0;
     long lastUse = 0;
     long hits = 0;
     cudaGraphExec_t graphExec = nullptr;      // the plan's phase launches as one graph launch (plans with >= 2 launches)
@@ -200,7 +206,6 @@ struct Instance {
     int lookaheadPre = 1;                     // look-ahead prefetch in pre-order walks too (B200_LOOKAHEAD_PRE)
     int prePhases = 1;                        // pre-order lists as phased subtree walks (0: one launch per depth level)
     int useGraphs = 1;                        // B200_GRAPHS
-    int lookahead = 1;                        // L1 prefetch of the next op's operands (B200_LOOKAHEAD)
     int forward = 1;                          // register forwarding between consecutive ops of a walk (B200_FORWARD)
     // slots per warp of the staged eigen walk's sibling stack (api.cu::assignStackSlots); B200_WALK_STACK_SLOTS=0 turns
     // it off, the reference route of the bit-equality tests
@@ -249,14 +254,12 @@ struct Instance {
 
     // tuning knobs (environment overridable, see api.cu)
     size_t genericSmemConfigured = 0, mmaSmemConfigured[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    int walkBlock = 128;
     std::vector<CachedPlan> planCache;
     int planCacheSize = 4;
     long planClock = 0;
     unsigned long bufferEpoch = 0;     // bumped whenever a buffer changes kind (tip <-> partials) or partitions change
     int reorder = 1;
     int thinR1 = 1;              // thin (latency-bound) phases of the 4-state walk use one pattern group per thread
-    int mmaWarps = 4;            // codon-size tensor walk: 4 warps single-buffered (default) or 8 warps double-buffered
     int genericMma = 1;          // S > 4: 1 = fp64 tensor-core block walk, 0 = FMA block walk
     int walkR = 4;               // patterns per thread in the 4-state walk (1, 2 or 4)
     int phaseTmin = 4, phaseOversub = 0, phaseSmall = 24;   // phaseSmall: a remainder this short runs as one launch
