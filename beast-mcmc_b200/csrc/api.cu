@@ -574,16 +574,17 @@ cudaError_t launchPlan(Instance* in, const PlanRecord& r, const void* dBlock, in
         const int s0 = r.phaseStart[ph], s1 = r.phaseStart[ph + 1];
         if (s1 <= s0) continue;
         TimedScope ts(in, T_PARTIALS);
-        if (eigenSlot >= 0) {
-            e = launchWalk4E(in, static_cast<const Op4*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow, !r.byPartition,
-                             in->hEigen.data() + (size_t)eigenSlot * 36, dVirtTips,
-                             ph < r.phaseSlots.size() ? r.phaseSlots[ph] : 0);
+        if (!r.fourPath) {
+            e = launchWalkGeneric(in, static_cast<const DevOp*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow, r.preOrder);
             continue;
         }
-        if (dVirtTips != nullptr) return cudaErrorInvalidValue;          // no other walk reads virtual cherries
-        e = r.fourPath ? launchWalk4(in, static_cast<const Op4*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow, r.preOrder)
-                       : launchWalkGeneric(in, static_cast<const DevOp*>(dBlock), dSubs + s0, s1 - s0, r.maxWindow,
-                                           r.preOrder);
+        const Walk4Route route = walk4Route(in, s1 - s0, r.maxWindow, eigenSlot >= 0, !r.byPartition, r.readsVirtual);
+        if (route.kernel == Walk4Kernel::Unservable) return cudaErrorInvalidValue;
+        const Op4* ops = static_cast<const Op4*>(dBlock);
+        e = eigenSlot >= 0 ? launchWalk4E(in, route, ops, dSubs + s0, s1 - s0, r.maxWindow,
+                                          in->hEigen.data() + (size_t)eigenSlot * 36, dVirtTips,
+                                          ph < r.phaseSlots.size() ? r.phaseSlots[ph] : 0)
+                           : launchWalk4(in, route, ops, dSubs + s0, s1 - s0, r.maxWindow, r.preOrder);
     }
     return e;
 }
@@ -823,9 +824,9 @@ void encodeDevOp(const Instance* in, const HostOp& o, int pBegin, int pEnd, DevO
 // only where the phase is throughput-bound; a thin phase is a pure latency chain and the extra instructions cost
 // more than the prefetch gives (measured on the 62-taxon benchmark2 alignment: +17 % with, in thin phases)
 void setLookahead(const Instance* in, std::vector<Op4>& ops, const Plan& plan, int maxWindow) {
-    const long perSub = (maxWindow + (32 / in->matCP) * in->walkR - 1) / ((32 / in->matCP) * in->walkR);
     for (size_t ph = 0; ph + 1 < plan.phaseStart.size(); ++ph) {
-        if ((long)(plan.phaseStart[ph + 1] - plan.phaseStart[ph]) * perSub < (long)in->smCount * 8) continue;
+        const int nSubs = plan.phaseStart[ph + 1] - plan.phaseStart[ph];
+        if (walk4Route(in, nSubs, maxWindow, false, false, false).thin) continue;     // thin is the same in either form
         for (int q = plan.phaseStart[ph]; q < plan.phaseStart[ph + 1]; ++q)
             for (int pos = plan.subs[q].begin; pos + 1 < plan.subs[q].end; ++pos) {
                 Op4& d = ops[pos];
@@ -868,7 +869,8 @@ std::vector<char> buildPlan(const Instance* in, const std::vector<HostOp>& hops,
         bool served = true;
         for (size_t ph = 0; r.readsVirtual && ph + 1 < plan.phaseStart.size(); ++ph) {
             const int nSubs = plan.phaseStart[ph + 1] - plan.phaseStart[ph];
-            served = served && (nSubs == 0 || walk4pServes(in, nSubs, in->Ppad));
+            served = served &&
+                     (nSubs == 0 || walk4Route(in, nSubs, in->Ppad, true, true, true).kernel != Walk4Kernel::Unservable);
         }
         if (!served) {
             r.readsVirtual = false;
@@ -2357,6 +2359,20 @@ int b200DebugStackSlots(const int* operations, int operationCount, int bufferCou
     outCounts[2] = (int)fromStack;
     outCounts[3] = (int)fromMemory;
     outCounts[4] = *std::max_element(subDepth.begin(), subDepth.end());
+    return BEAGLE_SUCCESS;
+}
+
+// ---- host-logic test hook (no CUDA calls): the 4-state walk kernel, R and thinness of a phase ---------------------------
+int b200DebugWalkRoute(int matCP, int Ppad, int smCount, int walkR, int thinR1, int single, int nSubs, int maxWindow,
+                       int eigenForm, int aligned, int virt, int* outRoute) {
+    const bool cpOk = matCP == 1 || matCP == 2 || matCP == 4 || matCP == 8 || matCP == 16 || matCP == 32;
+    if (!cpOk || (walkR != 1 && walkR != 2 && walkR != 4) || Ppad <= 0 || smCount <= 0 || nSubs < 0 || maxWindow <= 0 ||
+        outRoute == nullptr)
+        return BEAGLE_ERROR_OUT_OF_RANGE;
+    Instance in;
+    in.matCP = matCP; in.Ppad = Ppad; in.smCount = smCount; in.walkR = walkR; in.thinR1 = thinR1; in.single = single != 0;
+    const Walk4Route r = walk4Route(&in, nSubs, maxWindow, eigenForm != 0, aligned != 0, virt != 0);
+    outRoute[0] = (int)r.kernel; outRoute[1] = r.R; outRoute[2] = r.thin;
     return BEAGLE_SUCCESS;
 }
 

@@ -275,20 +275,39 @@ int shardedCreate(Instance* parent, int g, const int* devices, int tipCount, int
                   int scaleBufferCount, long preferenceFlags, long requirementFlags, void* details /* BeagleInstanceDetails* */);
 void shardedDestroy(Instance* parent);
 
+// ---- the 4-state walk kernel of a phase (walk4e.cu; no CUDA calls) ----------------------------------------------------
+// The planner and both launchers ask walk4Route, so the choice is stated once.  Values are those of b200DebugWalkRoute.
+enum class Walk4Kernel {
+    Matrix = 0,           // k_walk4 / k_walk4s (kernels.cu): matrix form
+    EigenPredicated = 1,  // k_walk4e<CP, R, false> / k_walk4es: eigen form, per-pattern predicates
+    EigenAligned = 2,     // k_walk4e<CP, R, true>: eigen form without predicates (CP 16, 32)
+    Staged = 3,           // k_walk4p / k_walk4ps: eigen form, per-warp asynchronous operand staging
+    StagedVirtual = 4,    // k_walk4pv / k_walk4pvs: staged, the records name virtual cherries
+    Unservable = 5,       // no kernel is built for the phase
+};
+struct Walk4Route {
+    Walk4Kernel kernel;
+    int R;                // patterns per thread
+    bool thin;            // few walks in flight: the phase is latency-bound
+};
+// a phase of nSubs subtree walks over at most maxWindow patterns; eigenForm: the list runs in eigen form (else matrix
+// form); aligned: every op covers [0, Ppad); virt: the records name virtual cherries
+Walk4Route walk4Route(const Instance* in, int nSubs, int maxWindow, bool eigenForm, bool aligned, bool virt);
+
 // ---- kernel launchers (kernels.cu) -----------------------------------------------------------
 cudaError_t launchTransitionMatrices(Instance* in, const int* dProbIdx, const int* dEigenIdx,
                                      const int* dRateSet, const double* dLengths, int count);
-// dSubs[k] = (first op, one-past-last op, first pattern, one-past-last pattern) of subtree walk k
-cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder);
-// walk4e.cu: eigen-form 4-state walk; eigen = [V (16) | V^-1 (16)]; aligned = every op covers [0, Ppad)
+// matrix-form 4-state walk of one phase on route.kernel == Matrix; dSubs[k] = (first op, one-past-last op, first pattern,
+// one-past-last pattern) of subtree walk k
+cudaError_t launchWalk4(Instance* in, const Walk4Route& route, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow,
+                        bool preOrder);
+// walk4e.cu: eigen-form 4-state walk; eigen = [V (16) | V^-1 (16)]
 // new V | V^-1 (32 doubles) for the captured eigen-form walk launches of a graph; any failure = the caller re-captures
 cudaError_t updateWalk4EGraph(cudaGraphExec_t exec, const std::vector<cudaGraphNode_t>& kernelNodes, const double* eigen);
-// dVirtTips non-null: the records name virtual cherries whose tips are dVirtTips[op] (an error unless every phase runs on
-// k_walk4p, see walk4pServes); stackSlots: slots per warp of the sibling stack the records use (k_walk4p only, 0 = none)
-cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
+// one phase on an eigen-form route; dVirtTips: the tips of the virtual cherries the records name, dVirtTips[op] (route
+// StagedVirtual only); stackSlots: slots per warp of the sibling stack the records use (staged routes only, 0 = none)
+cudaError_t launchWalk4E(Instance* in, const Walk4Route& route, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow,
                          const double* eigen, const int4* dVirtTips, int stackSlots);
-// whether an aligned eigen-form phase of nSubs subtree walks runs on k_walk4p (the kernel that reads virtual cherries)
-bool walk4pServes(const Instance* in, int nSubs, int maxWindow);
 // whether the staged-walk kernels this instance launches carry the sibling stack (otherwise they ignore the slot bytes)
 bool walkStackBuilt(const Instance* in);
 // recipe rows of the virtual cherries a list produces: items (buffer, m1, m2, -)

@@ -542,53 +542,45 @@ k_walk4s(const WalkArgs A) {
     walk4Body<float, CP, R, PRE>(A);
 }
 
-template <int CP, int R, bool PRE>
-static cudaError_t launchWalk4K(Instance* in, const WalkArgs& A, dim3 grid) {
-    if (in->single) {
-        if constexpr (CP <= 8) k_walk4s<CP, R, PRE><<<grid, 128, 0, in->stream>>>(A);
-        else return cudaErrorInvalidValue;
-        return cudaGetLastError();
+// fp32 storage is built for CP <= 8 only (single instances have C <= 8; walk4Route turns the others away)
+template <int CP, int R>
+static cudaError_t launchMatrixWalk(Instance* in, const WalkArgs& A, dim3 grid, bool preOrder) {
+    if (!in->single) {
+        if (preOrder) k_walk4<CP, R, true><<<grid, 128, 0, in->stream>>>(A);
+        else k_walk4<CP, R, false><<<grid, 128, 0, in->stream>>>(A);
+    } else if constexpr (CP <= 8) {
+        if (preOrder) k_walk4s<CP, R, true><<<grid, 128, 0, in->stream>>>(A);
+        else k_walk4s<CP, R, false><<<grid, 128, 0, in->stream>>>(A);
+    } else {
+        return cudaErrorInvalidValue;
     }
-    k_walk4<CP, R, PRE><<<grid, 128, 0, in->stream>>>(A);
     return cudaGetLastError();
 }
 
-template <int CP, int R>
-static cudaError_t launchWalk4R(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
-    constexpr int G = 32 / CP;
-    const int warps = (maxWindow + G * R - 1) / (G * R);
-    dim3 grid((warps + 3) / 4, nSubs);
-    WalkArgs A;
-    A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
-    A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
-    A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
-    A.matStride = in->matStride;
-    if (preOrder) return launchWalk4K<CP, R, true>(in, A, grid);
-    return launchWalk4K<CP, R, false>(in, A, grid);
-}
-
-template <int CP>
-static cudaError_t launchWalk4T(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
-    // a thin phase (few walks in flight) is latency-bound: one pattern group per thread gives 4x the warps per op
-    const long walks = (long)nSubs * ((maxWindow + (32 / CP) * in->walkR - 1) / ((32 / CP) * in->walkR));
-    if (in->thinR1 && walks < (long)in->smCount * 8)
-        return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-    switch (in->walkR) {
-        case 4: return launchWalk4R<CP, 4>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        case 2: return launchWalk4R<CP, 2>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        default: return launchWalk4R<CP, 1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-    }
-}
-
-cudaError_t launchWalk4(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool preOrder) {
-    if (nSubs <= 0) return cudaSuccess;
-    switch (in->matCP) {
-        case 1: return launchWalk4T<1>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        case 2: return launchWalk4T<2>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        case 4: return launchWalk4T<4>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        case 8: return launchWalk4T<8>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        case 16: return launchWalk4T<16>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
-        default: return launchWalk4T<32>(in, dOps, dSubs, nSubs, maxWindow, preOrder);
+cudaError_t launchWalk4(Instance* in, const Walk4Route& route, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow,
+                        bool preOrder) {
+    const WalkArgs A = walkArgs(in, dOps, dSubs);
+    const dim3 grid = walkGrid(in->matCP, route.R, nSubs, maxWindow);
+    switch (in->matCP * 8 + route.R) {                             // (CP, R)
+        case 1 * 8 + 1: return launchMatrixWalk<1, 1>(in, A, grid, preOrder);
+        case 1 * 8 + 2: return launchMatrixWalk<1, 2>(in, A, grid, preOrder);
+        case 1 * 8 + 4: return launchMatrixWalk<1, 4>(in, A, grid, preOrder);
+        case 2 * 8 + 1: return launchMatrixWalk<2, 1>(in, A, grid, preOrder);
+        case 2 * 8 + 2: return launchMatrixWalk<2, 2>(in, A, grid, preOrder);
+        case 2 * 8 + 4: return launchMatrixWalk<2, 4>(in, A, grid, preOrder);
+        case 4 * 8 + 1: return launchMatrixWalk<4, 1>(in, A, grid, preOrder);
+        case 4 * 8 + 2: return launchMatrixWalk<4, 2>(in, A, grid, preOrder);
+        case 4 * 8 + 4: return launchMatrixWalk<4, 4>(in, A, grid, preOrder);
+        case 8 * 8 + 1: return launchMatrixWalk<8, 1>(in, A, grid, preOrder);
+        case 8 * 8 + 2: return launchMatrixWalk<8, 2>(in, A, grid, preOrder);
+        case 8 * 8 + 4: return launchMatrixWalk<8, 4>(in, A, grid, preOrder);
+        case 16 * 8 + 1: return launchMatrixWalk<16, 1>(in, A, grid, preOrder);
+        case 16 * 8 + 2: return launchMatrixWalk<16, 2>(in, A, grid, preOrder);
+        case 16 * 8 + 4: return launchMatrixWalk<16, 4>(in, A, grid, preOrder);
+        case 32 * 8 + 1: return launchMatrixWalk<32, 1>(in, A, grid, preOrder);
+        case 32 * 8 + 2: return launchMatrixWalk<32, 2>(in, A, grid, preOrder);
+        case 32 * 8 + 4: return launchMatrixWalk<32, 4>(in, A, grid, preOrder);
+        default: return cudaErrorInvalidValue;
     }
 }
 

@@ -74,6 +74,22 @@ struct WalkArgs {
     double Vi[16];             // Ievc[k][j]
 };
 
+// the fields both forms fill from the instance (the eigen form adds its own)
+inline WalkArgs walkArgs(const Instance* in, const Op4* dOps, const int4* dSubs) {
+    WalkArgs A;
+    A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
+    A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
+    A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
+    A.matStride = in->matStride;
+    return A;
+}
+
+// 128-thread blocks of 4 warps, a warp per 32 / CP * R patterns of the window; one grid row per subtree walk
+inline dim3 walkGrid(int CP, int R, int nSubs, int maxWindow) {
+    const int G = 32 / CP, warps = (maxWindow + G * R - 1) / (G * R);
+    return dim3((warps + 3) / 4, nSubs);
+}
+
 __device__ __forceinline__ Op4 loadOp(const Op4* p) {
     const int4* q = reinterpret_cast<const int4*>(p);
     int4 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);

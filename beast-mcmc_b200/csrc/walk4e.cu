@@ -554,14 +554,33 @@ cudaError_t launchStaged(Instance* in, const WalkArgs& A, dim3 grid, int stackSl
     return cudaGetLastError();
 }
 
-template <typename T, int CP, int R>
-cudaError_t launchP(Instance* in, const WalkArgs& A, dim3 grid, int stackSlots, bool virt) {
-    if (virt) {
-        if constexpr (sizeof(T) == 4) return launchStaged<k_walk4pvs<CP, R>, CP, R>(in, A, grid, stackSlots);
-        else return launchStaged<k_walk4pv<CP, R>, CP, R>(in, A, grid, stackSlots);
+// the kernel of one (CP, R) for the route's family and the instance's precision: the staged kernels and fp32 storage are
+// built for CP <= 8, the ALIGNED k_walk4e for CP 16 and 32
+template <int CP, int R>
+cudaError_t launchEigenWalk(Instance* in, Walk4Kernel kernel, const WalkArgs& A, dim3 grid, int stackSlots) {
+    const bool s = in->single;
+    if constexpr (CP <= 8) {
+        switch (kernel) {
+            case Walk4Kernel::Staged:
+                return s ? launchStaged<k_walk4ps<CP, R>, CP, R>(in, A, grid, stackSlots)
+                         : launchStaged<k_walk4p<CP, R>, CP, R>(in, A, grid, stackSlots);
+            case Walk4Kernel::StagedVirtual:
+                return s ? launchStaged<k_walk4pvs<CP, R>, CP, R>(in, A, grid, stackSlots)
+                         : launchStaged<k_walk4pv<CP, R>, CP, R>(in, A, grid, stackSlots);
+            case Walk4Kernel::EigenPredicated:
+                if (s) k_walk4es<CP, R, false><<<grid, 128, 0, in->stream>>>(A);
+                else k_walk4e<CP, R, false><<<grid, 128, 0, in->stream>>>(A);
+                return cudaGetLastError();
+            default: return cudaErrorInvalidValue;
+        }
+    } else {
+        if (s) return cudaErrorInvalidValue;
+        switch (kernel) {
+            case Walk4Kernel::EigenAligned: k_walk4e<CP, R, true><<<grid, 128, 0, in->stream>>>(A); return cudaGetLastError();
+            case Walk4Kernel::EigenPredicated: k_walk4e<CP, R, false><<<grid, 128, 0, in->stream>>>(A); return cudaGetLastError();
+            default: return cudaErrorInvalidValue;
+        }
     }
-    if constexpr (sizeof(T) == 4) return launchStaged<k_walk4ps<CP, R>, CP, R>(in, A, grid, stackSlots);
-    else return launchStaged<k_walk4p<CP, R>, CP, R>(in, A, grid, stackSlots);
 }
 
 // recipe rows [buffer][2][16 * CP] of the virtual cherries a list produces: items (buffer, m1, m2, -)
@@ -607,95 +626,55 @@ __global__ void k_cherry_store_f32(const int4* items, int count, float* partials
     cherryStoreBody(items, count, partials, stride, states, recipes, S, C, CP, Ppad);
 }
 
-template <typename T, int CP, int R, bool ALIGNED>
-cudaError_t launchK(Instance* in, const WalkArgs& A, dim3 grid) {
-    if constexpr (sizeof(T) == 4) k_walk4es<CP, R, ALIGNED><<<grid, 128, 0, in->stream>>>(A);
-    else k_walk4e<CP, R, ALIGNED><<<grid, 128, 0, in->stream>>>(A);
-    return cudaGetLastError();
-}
-
-// patterns per thread of a phase: a thin phase (few walks in flight) is latency-bound, one pattern group per thread gives
-// the most warps per op; R = 2 is built for CP = 4 only
-int phaseR(const Instance* in, int nSubs, int maxWindow) {
-    const int G = 32 / in->matCP;
-    const long walks = (long)nSubs * ((maxWindow + G * in->walkR - 1) / (G * in->walkR));
-    if ((in->thinR1 && walks < (long)in->smCount * 8) || in->walkR == 1) return 1;
-    if (in->matCP == 4 && in->walkR == 2) return 2;
-    return 4;
-}
-
-bool stagedWalk(const Instance* in, int R, bool aligned) {
-    const int G = 32 / in->matCP;
-    // predicate-free only when a warp's G*R patterns can never straddle the end of the padded pattern axis
-    return aligned && in->Ppad % (G * R) == 0 && in->matCP <= 8 && G * R >= 4;
-}
-
-// stackSlots: slots per warp of the phase's sibling stack (0 = none)
-template <typename T, int CP, int R>
-cudaError_t launchR(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt, int stackSlots) {
-    constexpr int G = 32 / CP;
-    const int warps = (maxWindow + G * R - 1) / (G * R);
-    dim3 grid((warps + 3) / 4, nSubs);
-    if constexpr (CP <= 8 && G * R >= 4) {
-        // per-warp asynchronous operand staging (k_walk4p): every aligned list at CP <= 8, since G * R >= 4 there
-        if (stagedWalk(in, R, aligned)) return launchP<T, CP, R>(in, A, grid, stackSlots, virt);
-    }
-    if (virt) return cudaErrorInvalidValue;                        // only k_walk4p reads virtual cherries
-    if constexpr (CP > 8) {
-        if (aligned && in->Ppad % (G * R) == 0) return launchK<T, CP, R, true>(in, A, grid);
-    }
-    return launchK<T, CP, R, false>(in, A, grid);
-}
-
-template <typename T, int CP>
-cudaError_t launchCP(Instance* in, WalkArgs& A, int nSubs, int maxWindow, bool aligned, bool virt, int stackSlots) {
-    const int R = phaseR(in, nSubs, maxWindow);
-    if (R == 1) return launchR<T, CP, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-    if constexpr (CP == 4) {
-        if (R == 2) return launchR<T, CP, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-    }
-    return launchR<T, CP, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-}
-
 }  // namespace
 
 bool walkStackBuilt(const Instance* in) { return stackBuilt(in->matCP); }
 
-bool walk4pServes(const Instance* in, int nSubs, int maxWindow) {
-    if (in->matCP == 0) return false;
-    return stagedWalk(in, phaseR(in, nSubs, maxWindow), true);
+Walk4Route walk4Route(const Instance* in, int nSubs, int maxWindow, bool eigenForm, bool aligned, bool virt) {
+    const int CP = in->matCP, G = 32 / CP;
+    // a thin phase (few walks in flight) is latency-bound: one pattern group per thread gives the most warps per op
+    const long walks = (long)nSubs * ((maxWindow + G * in->walkR - 1) / (G * in->walkR));
+    Walk4Route r{Walk4Kernel::Unservable, in->walkR, walks < (long)in->smCount * 8};
+    if (in->thinR1 && r.thin) r.R = 1;
+    else if (eigenForm && r.R > 1) r.R = CP == 4 && in->walkR == 2 ? 2 : 4;     // the eigen form builds R = 2 at CP = 4 only
+    if (in->single && CP > 8) return r;                  // fp32 storage is built for CP <= 8 (single instances have C <= 8)
+    if (!eigenForm) {
+        if (!virt) r.kernel = Walk4Kernel::Matrix;       // only the staged eigen-form kernels read virtual cherries
+        return r;
+    }
+    // predicate-free only when a warp's G * R patterns can never straddle the end of the padded pattern axis; the staged
+    // kernels need at least 4 patterns per warp
+    const bool whole = aligned && in->Ppad % (G * r.R) == 0;
+    if (whole && CP <= 8 && G * r.R >= 4) r.kernel = virt ? Walk4Kernel::StagedVirtual : Walk4Kernel::Staged;
+    else if (!virt) r.kernel = whole && CP > 8 ? Walk4Kernel::EigenAligned : Walk4Kernel::EigenPredicated;
+    return r;
 }
 
 // eigen: [V (16, row-major Evec[i][k]) | V^-1 (16, Ievc[k][j])], padded to 4 x 4 with zeros
-cudaError_t launchWalk4E(Instance* in, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow, bool aligned,
+cudaError_t launchWalk4E(Instance* in, const Walk4Route& route, const Op4* dOps, const int4* dSubs, int nSubs, int maxWindow,
                          const double* eigen, const int4* dVirtTips, int stackSlots) {
-    const bool virt = dVirtTips != nullptr;
-    if (nSubs <= 0) return cudaSuccess;
-    WalkArgs A;
-    A.ops = dOps; A.subs = dSubs; A.partials = in->partialsBase; A.stride = in->partialsElems;
-    A.states = in->states8Base; A.mats = in->dMat; A.scale = in->dScale;
-    A.S = in->S; A.C = in->C; A.Ppad = in->Ppad; A.logScalers = in->logScalers ? 1 : 0;
-    A.matStride = in->matStride;
+    if (route.kernel == Walk4Kernel::StagedVirtual && in->dRecipe == nullptr) return cudaErrorInvalidValue;
+    WalkArgs A = walkArgs(in, dOps, dSubs);
     A.evecs = in->dEvec;
     A.recipes = in->dRecipe;
     A.virtTips = dVirtTips;
-    if (virt && in->dRecipe == nullptr) return cudaErrorInvalidValue;
     for (int q = 0; q < 16; ++q) { A.V[q] = eigen[q]; A.Vi[q] = eigen[16 + q]; }
-    if (in->single) {                                // CP <= 8 only: single instances have C <= 8
-        switch (in->matCP) {
-            case 1: return launchCP<float, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-            case 2: return launchCP<float, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-            case 8: return launchCP<float, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-            default: return launchCP<float, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        }
-    }
-    switch (in->matCP) {
-        case 1: return launchCP<double, 1>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        case 2: return launchCP<double, 2>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        case 8: return launchCP<double, 8>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        case 16: return launchCP<double, 16>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        case 32: return launchCP<double, 32>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
-        default: return launchCP<double, 4>(in, A, nSubs, maxWindow, aligned, virt, stackSlots);
+    const dim3 grid = walkGrid(in->matCP, route.R, nSubs, maxWindow);
+    switch (in->matCP * 8 + route.R) {                             // (CP, R)
+        case 1 * 8 + 1: return launchEigenWalk<1, 1>(in, route.kernel, A, grid, stackSlots);
+        case 1 * 8 + 4: return launchEigenWalk<1, 4>(in, route.kernel, A, grid, stackSlots);
+        case 2 * 8 + 1: return launchEigenWalk<2, 1>(in, route.kernel, A, grid, stackSlots);
+        case 2 * 8 + 4: return launchEigenWalk<2, 4>(in, route.kernel, A, grid, stackSlots);
+        case 4 * 8 + 1: return launchEigenWalk<4, 1>(in, route.kernel, A, grid, stackSlots);
+        case 4 * 8 + 2: return launchEigenWalk<4, 2>(in, route.kernel, A, grid, stackSlots);
+        case 4 * 8 + 4: return launchEigenWalk<4, 4>(in, route.kernel, A, grid, stackSlots);
+        case 8 * 8 + 1: return launchEigenWalk<8, 1>(in, route.kernel, A, grid, stackSlots);
+        case 8 * 8 + 4: return launchEigenWalk<8, 4>(in, route.kernel, A, grid, stackSlots);
+        case 16 * 8 + 1: return launchEigenWalk<16, 1>(in, route.kernel, A, grid, stackSlots);
+        case 16 * 8 + 4: return launchEigenWalk<16, 4>(in, route.kernel, A, grid, stackSlots);
+        case 32 * 8 + 1: return launchEigenWalk<32, 1>(in, route.kernel, A, grid, stackSlots);
+        case 32 * 8 + 4: return launchEigenWalk<32, 4>(in, route.kernel, A, grid, stackSlots);
+        default: return cudaErrorInvalidValue;
     }
 }
 

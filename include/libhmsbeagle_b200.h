@@ -498,6 +498,14 @@ BEAGLE_DLLEXPORT int b200DebugStackSlots(const int* operations, int operationCou
                                          int wantSubs, int minT, int smallRemainder, int* outRecords, int* outSubs,
                                          int* outPhaseStart, int* outCounts);
 
+/* Host-logic test hook (no CUDA): the 4-state walk kernel of one phase of nSubs subtree walks over at most maxWindow
+ * patterns, on an instance with the given padded categories (1, 2, 4, 8, 16 or 32), padded pattern count, SM count,
+ * patterns per thread (1, 2 or 4), thin-phase rule and precision.  eigenForm: the list runs in eigen form; aligned: every
+ * op covers all patterns; virt: the records name virtual cherries.  outRoute = {kernel, R, thin}; kernel 0 = matrix form,
+ * 1 = eigen form with predicates, 2 = eigen form without, 3 = staged, 4 = staged with virtual cherries, 5 = no kernel. */
+BEAGLE_DLLEXPORT int b200DebugWalkRoute(int matCP, int Ppad, int smCount, int walkR, int thinR1, int single, int nSubs,
+                                        int maxWindow, int eigenForm, int aligned, int virt, int* outRoute);
+
 #ifdef __cplusplus
 }
 #endif

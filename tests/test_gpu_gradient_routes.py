@@ -233,10 +233,10 @@ R_ENV = {1: {}, 2: {"B200_WALK_R": "2", "B200_THIN_R1": "0"}, 4: {"B200_WALK_R":
 @pytest.mark.parametrize("R", [1, 2, 4])
 @pytest.mark.parametrize("C", CATS)
 def test_preorder4_every_cp_and_r(C, R, P):
-    """Route: 4-state pre-order walk k_walk4<CP, R, true> (kernels.cu launchWalk4 -> launchWalk4T<CP>), CP =
+    """Route: 4-state pre-order walk k_walk4<CP, R, true> (kernels.cu launchWalk4 on the route of walk4Route), CP =
     matCP = C rounded up to a power of two (beagleCreateInstance); C = 40 has matCP = 0 and takes k_walk_generic
     (launchWalkGeneric, Sp = 4).  R = 1: the default rule of beagleCreateInstance halves walkR while a subtree has fewer
-    warps than SMs, and launchWalk4T's thin rule (walks < smCount * 8) picks R = 1 anyway.  R = 2 / 4: B200_WALK_R
+    warps than SMs, and walk4Route's thin rule (walks < smCount * 8) picks R = 1 anyway.  R = 2 / 4: B200_WALK_R
     forces walkR and B200_THIN_R1=0 disables the thin rule.  P = 301 leaves a partial last tile for every 32/CP * R,
     P = 1 a tile with one live pattern."""
     tw = Twin(4, C, 12, P, seed=100 + C + R, env=R_ENV[R])
@@ -254,7 +254,7 @@ def test_preorder4_every_cp_and_r(C, R, P):
 def test_preorder4_natural_r4(C, tips, P):
     """Route: k_walk4<CP, 4, true> by the default rules alone: walkR stays 4 in beagleCreateInstance because
     Ppad / (32/CP * 4) >= smCount (1250 warps at CP = 4, 500 at CP = 32), and the phases of planPreorderPhases are wide
-    enough that launchWalk4T's thin rule (walks < smCount * 8) does not apply."""
+    enough that walk4Route's thin rule (walks < smCount * 8) does not apply."""
     tw = Twin(4, C, tips, P, seed=7 + C, partialTips=0.1)
     try:
         lg, lo = tw.post_order()
