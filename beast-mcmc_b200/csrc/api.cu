@@ -579,6 +579,9 @@ cudaError_t launchPlan(Instance* in, const PlanRecord& r, const void* dBlock, in
             continue;
         }
         const Walk4Route route = walk4Route(in, s1 - s0, r.maxWindow, eigenSlot >= 0, !r.byPartition, r.readsVirtual);
+        if (in->debugLog)      // a graph replay does not come through here: its phases were logged at capture
+            fprintf(stderr, "[b200-beagle] phase %zu: %d walks over %d patterns, kernel %d, R %d, %s\n", ph, s1 - s0,
+                    r.maxWindow, (int)route.kernel, route.R, route.thin ? "thin" : "wide");
         if (route.kernel == Walk4Kernel::Unservable) return cudaErrorInvalidValue;
         const Op4* ops = static_cast<const Op4*>(dBlock);
         e = eigenSlot >= 0 ? launchWalk4E(in, route, ops, dSubs + s0, s1 - s0, r.maxWindow,
@@ -932,8 +935,8 @@ std::vector<char> buildPlan(const Instance* in, const std::vector<HostOp>& hops,
         int fwd = 0, internal = 0;
         for (const Op4& d : ops4) { fwd += (d.pad_ & 2) != 0; internal += (d.c1 >= 0) + (d.c2 >= 0); }
         fprintf(stderr, "[b200-beagle] plan: %d ops (%zu virtual cherries), %zu subtrees, %d phases, %d internal children, "
-                "%d forwarded in registers, %ld read from the stack, %ld from memory\n", nL, r.cherries.size(), plan.subs.size(),
-                nPhases, internal, fwd, fromStack, fromMemory);
+                "%d forwarded in registers, %ld read from the stack, %ld from memory, walkR %d\n", nL, r.cherries.size(),
+                plan.subs.size(), nPhases, internal, fwd, fromStack, fromMemory, in->walkR);
     }
     auto aligned = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
     const size_t opBytes = (r.fourPath ? sizeof(Op4) : sizeof(DevOp)) * (size_t)nL;
